@@ -9,6 +9,7 @@ PLACE_SELF, PLACE_HRW, PLACE_HRW2 = 0, 1, 2
 SOLVER_HRW, SOLVER_HRW2 = 1, 2
 EV_JOIN, EV_LEAVE = 1, 2
 COMM_ID_BYTES = 128
+MAX_RANKS = 8
 
 _lib = None
 
@@ -59,6 +60,8 @@ SIGNATURES = {
     "rio_cuda_directory_len": (C.c_int32, [H, u64p, u64p]),
     "rio_cuda_assign_batch": (C.c_int32, [H, vp, vp, sz, vp]),
     "rio_cuda_assign_bounded_batch": (C.c_int32, [H, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p]),
+    "rio_cuda_assign_ranked_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
+    "rio_cuda_assign_ranked_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_check_address_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp, u64p]),
     "rio_cuda_place_batch": (C.c_int32, [H, vp, sz, C.c_uint32, C.c_uint32, vp]),
     "rio_cuda_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),

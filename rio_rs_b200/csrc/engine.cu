@@ -7,6 +7,7 @@
 #include "../../include/rio_cuda.h"
 #include "../../include/rio_cuda_dev.h"
 #include "kernels.cuh"
+#include "k_ranked.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -179,6 +180,11 @@ struct rio_placement {
     BoundedState bs;                          // for rio_cuda_assign_bounded_batch (host buffers)
     uint64_t tab_version = 0;
     uint64_t live_sig = 0;                    // live_signature() of the node set the current table was built from
+    // side table of the ranked HRW2 walk (DESIGN.md 3.9): built on the first ranked call after a table change, never by other calls
+    DevBuf rank_dev;
+    std::vector<unsigned char> rank_stage;
+    TrieRankDev rank_tab{};
+    uint64_t rank_version = ~0ull;            // tab_version the side table belongs to
     unsigned long long *d_scalars = nullptr;   // S_COUNT u64 + error u32
     unsigned long long *h_scalars = nullptr;   // pinned mirror
 
@@ -488,6 +494,52 @@ void run_assign(rio_placement *h, uint32_t solver, const TabBufs &tb, const uint
                 const uint32_t *d_sel, uint64_t n_sel) {
     if (solver == RIO_SOLVER_HRW2) launch_assign_trie(h->L(), d_keys, n, tb.trie, d_out_idx, d_counters, d_sel, n_sel, tb.tab.n_total);
     else launch_assign_hrw(h->L(), d_keys, n, tb.tab, d_out_idx, d_counters, d_sel, n_sel);
+}
+
+// The ranked HRW2 walk needs, beside the blob, the subtree weights the thresholds came from and every live node's bucket and
+// weight.  The builder is run again for the current live set (a pure function of it: the same blob, and its weight heap).
+void ensure_rank_tab(rio_placement *h) {
+    if (h->rank_version == h->tab_version) return;
+    const uint32_t n_total = (uint32_t)h->nodes.size();
+    std::vector<TrieMember> members;
+    for (uint32_t j = 0; j < n_total; j++)
+        if (h->nodes[j].live()) members.push_back(TrieMember{h->nodes[j].seed, j, h->nodes[j].weight});
+    const TrieBlob blob = build_trie_blob(members, h->trie_bits);
+    const uint32_t bits = blob.bits, nb = 1u << bits;
+    const size_t o_node = (size_t)nb * 16, total = o_node + ((size_t)n_total * 8 + 15) / 16 * 16;
+    h->rank_stage.assign(total, 0);
+    memcpy(h->rank_stage.data(), blob.wsum.data(), (size_t)nb * 16);
+    uint2 *node = reinterpret_cast<uint2 *>(h->rank_stage.data() + o_node);
+    for (const TrieMember &m : members) {
+        const uint64_t pos = mix64(m.seed ^ kSaltPos);
+        node[m.idx] = make_uint2(bits ? (uint32_t)(pos >> (64 - bits)) : 0u, m.weight);
+    }
+    cudaStream_t st = h->stream;
+    h->rank_dev.ensure(total, st);
+    CUDA_TRY(cudaMemcpyAsync(h->rank_dev.p, h->rank_stage.data(), total, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    unsigned char *d = h->rank_dev.as<unsigned char>();
+    h->rank_tab = TrieRankDev{reinterpret_cast<const unsigned long long *>(d), reinterpret_cast<const uint2 *>(d + o_node), n_total,
+                              (uint32_t)members.size(), (uint32_t)total};
+    h->rank_version = h->tab_version;
+}
+
+void check_ranked_args(size_t n, uint32_t ranks) {
+    REQUIRE(ranks >= 1 && ranks <= RIO_MAX_RANKS, "ranks must be in [1, RIO_MAX_RANKS]");
+    REQUIRE(n <= SIZE_MAX / 4 / ranks, "n x ranks overflows");
+}
+
+// each object's first `ranks` distinct nodes under the handle's policy (DESIGN.md 3.9)
+void run_assign_ranked(rio_placement *h, const uint64_t *d_keys, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!launch_assign_hrw_ranked || !launch_assign_trie_ranked)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked kernels (k_ranked.cu is not linked)"};
+    ensure_tab(h);
+    if (h->solver == RIO_SOLVER_HRW2) {
+        ensure_rank_tab(h);
+        launch_assign_trie_ranked(h->L(), d_keys, n, h->tabs.trie, h->rank_tab, ranks, d_out_idx);
+    } else {
+        launch_assign_hrw_ranked(h->L(), d_keys, n, h->tabs.tab, ranks, d_out_idx);
+    }
 }
 
 // affinity dispatch: tensor-core (wgmma) kernel for K == 16 (unless RIO_AFFINITY_VARIANT=ffma or the node set does not fit), else CUDA cores
@@ -858,7 +910,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -1162,6 +1214,32 @@ rio_status rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, c
         } else {
             run_assign(h, h->solver, h->tabs, d_keys, n, d_out_idx, nullptr, nullptr, 0);
         }
+    });
+}
+
+rio_status rio_cuda_assign_ranked_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(keys && out_idx, "null buffer");
+        cudaStream_t st = h->stream;
+        h->s_keys.ensure(n * 8, st);
+        h->s_idx.ensure(n * ranks * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
+        run_assign_ranked(h, h->s_keys.as<uint64_t>(), n, ranks, h->s_idx.as<uint32_t>());
+        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    });
+}
+
+rio_status rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(d_keys && d_out_idx, "null buffer");
+        run_assign_ranked(h, d_keys, n, ranks, d_out_idx);
     });
 }
 

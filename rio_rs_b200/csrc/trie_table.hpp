@@ -35,6 +35,8 @@ struct TrieBlob {
     uint32_t off_crec = 0;         // byte offset of the first chain record
     uint32_t n_chain = 0;          // chain records
     uint32_t bits = 0;
+    std::vector<uint64_t> wsum;    // heap of subtree weights the thresholds were derived from (index 1 = root, buckets at [2^bits, 2^(bits+1)));
+                                   // not part of the blob: the ranked walk (DESIGN.md 3.9) re-derives the contests that exclusions change
 };
 
 // T3 of a contest (spec.cuh contest_t3) for the common case "both weights and their sum below 2^32": floor(2^31 wl / (wl + wr)) by one
@@ -112,6 +114,7 @@ inline TrieBlob build_trie_blob(const std::vector<TrieMember> &members, uint32_t
             d[5] = q + 2 == hi ? mem[hi - 1].idx : 0x80000000u | (rec_off + 32u);
         }
     }
+    b.wsum = std::move(wsum);
     return b;
 }
 

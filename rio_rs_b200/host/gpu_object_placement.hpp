@@ -115,6 +115,12 @@ class GpuObjectPlacement {
         check(rio_cuda_assign_batch(e_->h, keys.data(), nullptr, keys.size(), out.data()));
         return out;
     }
+    // each object's first `ranks` distinct nodes (DESIGN.md 3.9), row-major: object i's list at [i * ranks, (i + 1) * ranks)
+    std::vector<uint32_t> assign_ranked(const std::vector<uint64_t> &keys, uint32_t ranks) const {
+        std::vector<uint32_t> out(keys.size() * ranks);
+        check(rio_cuda_assign_ranked_batch(e_->h, keys.data(), keys.size(), ranks, out.data()));
+        return out;
+    }
     std::vector<uint32_t> place_batch(const std::vector<uint64_t> &keys, uint32_t policy, uint32_t self_idx) const {
         std::vector<uint32_t> out(keys.size());
         check(rio_cuda_place_batch(e_->h, keys.data(), keys.size(), policy, self_idx, out.data()));

@@ -263,6 +263,14 @@ class GpuObjectPlacement:
         self._ck(self.L.rio_cuda_assign_batch(self.h, _ptr(keys), _ptr(obj_feats), n, _ptr(out)))
         return out
 
+    def assign_ranked(self, keys, ranks):
+        """Each object's first `ranks` distinct nodes under the handle's policy (DESIGN.md 3.9) -> (n, ranks) uint32: column 0 is
+        assign_batch, column 1 the failover target (where a LEAVE of column 0 sends the object); RIO_NONE past the live set."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.empty((len(keys), ranks), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_assign_ranked_batch(self.h, _ptr(keys), len(keys), ranks, _ptr(out)))
+        return out
+
     def assign_bounded_batch(self, keys, n_total=0, cap_num=5, cap_den=4, max_rounds=4, out=None):
         """assign_batch + bounded-load rounds for host buffers; returns (indices, passes)."""
         keys = np.ascontiguousarray(keys, dtype=np.uint64)

@@ -139,6 +139,14 @@ impl GpuObjectPlacement {
         check(self.h(), unsafe { sys::rio_cuda_assign_batch(self.h(), keys.as_ptr(), ptr::null(), keys.len(), out.as_mut_ptr()) })?;
         Ok(out)
     }
+    /// Each object's first `ranks` distinct nodes under the handle's policy (DESIGN.md 3.9), row-major: object i's list is
+    /// `out[i * ranks..(i + 1) * ranks]`.  Rank 2 is the failover target: where a leave of rank 1 sends the object.
+    pub fn assign_ranked(&self, keys: &[u64], ranks: u32) -> Result<Vec<u32>, ObjectPlacementError> {
+        let len = keys.len().checked_mul(ranks as usize).ok_or_else(|| ObjectPlacementError::Unknown("n x ranks overflows".into()))?;
+        let mut out = vec![sys::RIO_NONE; len];
+        check(self.h(), unsafe { sys::rio_cuda_assign_ranked_batch(self.h(), keys.as_ptr(), keys.len(), ranks, out.as_mut_ptr()) })?;
+        Ok(out)
+    }
     /// Eager re-placement after a membership event (beside peer_to_peer.rs:170-191).
     pub fn rebalance(&self, join: bool, node_idx: u32) -> Result<u64, ObjectPlacementError> {
         let mut moved = 0u64;
