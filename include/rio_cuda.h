@@ -139,11 +139,17 @@ rio_status  rio_cuda_assign_bounded_batch(rio_placement *h, const uint64_t *keys
                                           uint32_t cap_den, uint32_t max_rounds, uint32_t *out_idx, uint32_t *out_passes);
 /* Ranked placement (DESIGN.md 3.9): each object's first `ranks` distinct nodes under the handle's solver policy.  rank 1 is
  * exactly what assign_batch returns; rank r is the same policy's placement over the live set minus ranks 1..r-1 -- so rank 2 is
- * where a LEAVE of rank 1 sends the object (its failover target).  Pure function of (keys, live set); hash path only.
+ * where a LEAVE of rank 1 sends the object (its failover target).  Pure function of (keys, live set); hash path only (the affinity cost: rio_cuda_assign_ranked_affinity_batch).
  * out_idx is n x ranks, row-major (object i's list at out_idx[i*ranks ..]); ranks beyond the live node count are RIO_NONE.
  * RIO_ERR_UNKNOWN for ranks outside [1, RIO_MAX_RANKS], NULL buffers, or n x ranks overflowing. */
 #define RIO_MAX_RANKS 8u
 rio_status  rio_cuda_assign_ranked_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx);
+/* Ranked placement under the affinity cost (DESIGN.md 3.9): each object's `ranks` lowest-cost live nodes, cost = -dot(F_obj, F_node),
+ * in increasing (cost, node index) order.  rank 1 is exactly what assign_batch with the same obj_feats returns; rank r is the
+ * affinity placement over the live set minus ranks 1..r-1, so rank 2 is where a LEAVE of rank 1 sends the object.  obj_feats is
+ * n x K (K of set_nodes), out_idx n x ranks row-major, RIO_NONE past the live node count.  RIO_ERR_UNKNOWN as for
+ * rio_cuda_assign_ranked_batch, and when the handle has no node features. */
+rio_status  rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx);
 /* Service::get_or_create_placement for a batch (service.rs:193-254): existing & live => keep; recorded on an
  * inactive node => clean_server(that node) then re-place; none => place.  policy RIO_PLACE_SELF re-places on
  * self_idx (the reference's rule, service.rs:244-252); RIO_PLACE_HRW / RIO_PLACE_HRW2 re-place by the solver. */
@@ -228,6 +234,7 @@ rio_status  rio_cuda_memcpy_d2h(rio_placement *h, void *host, const void *dev, s
 rio_status  rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, const float *d_obj_feats,
                                       size_t n, uint32_t *d_out_idx);
 rio_status  rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx);
+rio_status  rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_lookup_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t *d_out_idx);
 rio_status  rio_cuda_upsert_batch_dev(rio_placement *h, const uint64_t *d_keys, const uint32_t *d_idx, size_t n);
 /* pre-size the directory for n more distinct keys (the _dev upsert cannot grow it mid-stream) */

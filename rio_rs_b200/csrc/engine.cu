@@ -8,6 +8,7 @@
 #include "../../include/rio_cuda_dev.h"
 #include "kernels.cuh"
 #include "k_ranked.cuh"
+#include "k_affinity_ranked.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -554,6 +555,23 @@ void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d
         return;
     }
     launch_assign_affinity(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, d_out_idx, d_out_cost, d_counters);
+}
+
+// each object's `ranks` lowest-cost live nodes (DESIGN.md 3.9), on the path run_affinity takes for the same handle and environment,
+// so that rank 1 is its answer; the tensor-core pair keeps its per-object groups in s_idx2 between the two passes
+void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!launch_assign_affinity_ranked || !launch_assign_affinity_umma_ranked)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked affinity kernels (k_affinity_umma.cu / k_assign.cu are not linked)"};
+    const char *v = getenv("RIO_AFFINITY_VARIANT");
+    const bool want_umma = !(v && v[0] == 'f');
+    if (!h->aff_live && h->K == 16 && h->tabs.tab.n_live == 0) { launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); return; }
+    if (want_umma && h->K == 16 && h->aff_live && h->aff_pad <= affinity_umma_max_nodes()) {
+        h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
+        CUDA_TRY(launch_assign_affinity_umma_ranked(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(), h->aff_live,
+                                                    h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
+        return;
+    }
+    launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
 }
 
 uint32_t capacity_of(uint64_t n_total, uint32_t w, uint64_t w_sum, uint32_t num, uint32_t den) {
@@ -1240,6 +1258,37 @@ rio_status rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_
         if (!n) return;
         REQUIRE(d_keys && d_out_idx, "null buffer");
         run_assign_ranked(h, d_keys, n, ranks, d_out_idx);
+    });
+}
+
+rio_status rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(obj_feats && out_idx, "null buffer");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
+        ensure_tab(h);
+        cudaStream_t st = h->stream;
+        h->s_feats.ensure(n * h->K * 4, st);
+        h->s_idx.ensure(n * ranks * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, obj_feats, n * h->K * 4, cudaMemcpyHostToDevice, st));
+        run_affinity_ranked(h, h->s_feats.as<float>(), n, ranks, h->s_idx.as<uint32_t>());
+        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    });
+}
+
+rio_status rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(d_obj_feats && d_out_idx, "null buffer");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        ensure_tab(h);
+        run_affinity_ranked(h, d_obj_feats, n, ranks, d_out_idx);
     });
 }
 

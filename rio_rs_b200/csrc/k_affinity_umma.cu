@@ -21,6 +21,7 @@
 // k_affinity_resolve (second pass, CUDA cores) re-evaluates the 8 candidates of each winning group in fp32: node index +
 // fp32 cost + per-node histogram.
 #include "kernels.cuh"
+#include "k_affinity_ranked.cuh"
 #include "spec.cuh"
 
 #include <cuda_bf16.h>
@@ -318,6 +319,211 @@ k_affinity_resolve(const float *__restrict__ fobj, uint64_t n, const float *__re
     }
 }
 
+// ---- ranked lists (DESIGN.md 3.9) ------------------------------------------------------------------------------------------------
+// A row's list of RT (value, group) pairs, ordered by larger value, then smaller group; empty slots are (-inf, kNone).
+__device__ __forceinline__ bool group_before(float v, uint32_t g, float w, uint32_t h) { return v > w || (v == w && g < h); }
+
+// (v, g) into a list it beats at the last slot, behind every entry of equal value: the groups of a scan come in increasing order,
+// so this keeps "larger value, then smaller group", and with RT = 1 it is reduce_tile's update
+template <int RT>
+__device__ __forceinline__ void insert_scan(float (&lv)[RT], uint32_t (&lg)[RT], float v, uint32_t g) {
+#pragma unroll
+    for (int i = RT - 1; i > 0; i--) {
+        if (v > lv[i - 1]) { lv[i] = lv[i - 1]; lg[i] = lg[i - 1]; }
+        else if (v > lv[i]) { lv[i] = v; lg[i] = g; }
+    }
+    if (v > lv[0]) { lv[0] = v; lg[0] = g; }
+}
+
+// (v, g) from another lane's list: a group already present keeps the larger of its two values (a lane sees 2 of its 8 columns)
+template <int RT>
+__device__ __forceinline__ void insert_merge(float (&lv)[RT], uint32_t (&lg)[RT], float v, uint32_t g) {
+    bool dup = false;
+#pragma unroll
+    for (int i = 0; i < RT; i++)
+        if (lg[i] == g) { dup = true; lv[i] = fmaxf(lv[i], v); }
+    if (!dup && group_before(v, g, lv[RT - 1], lg[RT - 1])) { lv[RT - 1] = v; lg[RT - 1] = g; }
+#pragma unroll
+    for (int i = RT - 1; i > 0; i--)   // one entry is out of place at most: one bubble pass upwards restores the order
+        if (group_before(lv[i], lg[i], lv[i - 1], lg[i - 1])) {
+            const float tv = lv[i]; lv[i] = lv[i - 1]; lv[i - 1] = tv;
+            const uint32_t tg = lg[i]; lg[i] = lg[i - 1]; lg[i - 1] = tg;
+        }
+}
+
+// reduce_tile with a list of the best RT groups per row instead of the best one
+template <int NT, int RT>
+__device__ __forceinline__ void reduce_tile_ranked(float (&d)[NT / 2], uint32_t t, uint32_t q, uint32_t n_live, float (&lv)[2][RT], uint32_t (&lg)[2][RT]) {
+    const uint32_t col_base = t * NT;
+    if (col_base + NT > n_live) {
+#pragma unroll
+        for (int i = 0; i < NT / 2; i++)
+            if (col_base + 8 * (i >> 2) + 2 * q + (i & 1) >= n_live) d[i] = -INFINITY;
+    }
+#pragma unroll
+    for (int gi = 0; gi < NT / 8; gi++) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const float v = fmaxf(d[4 * gi + 2 * h], d[4 * gi + 2 * h + 1]);
+            if (v > lv[h][RT - 1]) insert_scan<RT>(lv[h], lg[h], v, (col_base >> 3) + gi);
+        }
+    }
+}
+
+// k_affinity_wgmma keeping each row's best RT distinct groups of 8 columns (a group's value: its largest column) in
+// out_groups[row * RT ..], kNone past the groups that hold live nodes.  Node staging, the A fragments and the six-term tiles are
+// k_affinity_wgmma's, so the accumulators are bit for bit the same and the first group is the one that kernel writes.  Each lane
+// keeps its own best RT over the 2 columns per group it holds; a group of the row's best RT has its value in some lane, and fewer
+// than RT groups beat it there, so merging the four lane lists (a butterfly over xor 1 and 2) finds the row's best RT.
+// WG warpgroups per CTA: the lists cost 4 RT registers per thread beside the 64 of the accumulator.
+template <int NT, int RT, int WG>
+__global__ void __launch_bounds__(128 * WG, 1) k_affinity_wgmma_ranked(WgmmaParams P) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    unsigned char *sB = smem;
+    const uint32_t b_block_bytes = P.m_pad * 32;
+    for (uint32_t p = threadIdx.x; p < P.m_pad; p += blockDim.x) {
+        float f[16];
+        const float4 *row = reinterpret_cast<const float4 *>(P.fnode_c + (size_t)p * 16);
+#pragma unroll
+        for (int q = 0; q < 4; q++) { const float4 v = __ldg(row + q); f[4 * q] = v.x; f[4 * q + 1] = v.y; f[4 * q + 2] = v.z; f[4 * q + 3] = v.w; }
+        store_row_split(sB, b_block_bytes, P.m_pad * 16, p, f);
+    }
+    fence_proxy_async();
+    __syncthreads();
+
+    const uint32_t wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const uint32_t q = lane & 3, r_in = warp * 16 + (lane >> 2);
+    const uint32_t n_tiles = P.m_pad / NT;
+    const uint64_t n_rb = (P.n + kRows - 1) / kRows, rb_step = (uint64_t)gridDim.x * WG;
+    const uint32_t sb = smem_u32(sB);
+
+    uint64_t rb = (uint64_t)blockIdx.x * WG + wg;
+    AFeat next = load_afeat(P.fobj, P.n, rb * kRows + r_in, q);
+    for (; rb < n_rb; rb += rb_step) {
+        const AFeat cur = next;
+        next = load_afeat(P.fobj, P.n, (rb + rb_step) * kRows + r_in, q);
+        uint32_t a[3][4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            __nv_bfloat16 h0, m0, l0, h1, m1, l1;
+            split3(cur.v[i].x, h0, m0, l0);
+            split3(cur.v[i].y, h1, m1, l1);
+            a[0][i] = pack2(h0, h1); a[1][i] = pack2(m0, m1); a[2][i] = pack2(l0, l1);
+        }
+        float lv[2][RT];
+        uint32_t lg[2][RT];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int i = 0; i < RT; i++) { lv[h][i] = -INFINITY; lg[h][i] = kNone; }
+        float acc[NT / 2];
+        for (uint32_t t = 0; t < n_tiles; t++) {
+            issue_tile<NT>(acc, a, sb, b_block_bytes, t, P.m_pad);
+            wgmma_wait<0>();
+            fence_regs(acc);
+            reduce_tile_ranked<NT, RT>(acc, t, q, P.n_live, lv, lg);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int d = 1; d <= 2; d <<= 1) {
+                float ov[RT];
+                uint32_t og[RT];
+#pragma unroll
+                for (int i = 0; i < RT; i++) { ov[i] = __shfl_xor_sync(0xFFFFFFFFu, lv[h][i], d); og[i] = __shfl_xor_sync(0xFFFFFFFFu, lg[h][i], d); }
+#pragma unroll
+                for (int i = 0; i < RT; i++) insert_merge<RT>(lv[h], lg[h], ov[i], og[i]);
+            }
+            const uint64_t row = rb * kRows + r_in + 8 * h;
+            if (q == 0 && row < P.n) {
+#pragma unroll
+                for (int i = 0; i < RT; i++) P.out_idx[row * RT + i] = lg[h][i];
+            }
+        }
+    }
+}
+
+// k_affinity_resolve over the RT groups of each object: lane 8q + r scores candidate r of every group of object q, with the same
+// fmaf order.  Rank 1 is the smallest (cost, position) of the first group, exactly as k_affinity_resolve picks it; ranks 2.. are
+// the smallest remaining (cost, position) over all 8 RT candidates.  Positions are compacted in node-index order, so this is
+// (cost, node index) order.  Each lane of an object holds one group index (lane r: group r), read by the others with a shuffle.
+// Launch bounds: without a minimum, ptxas keeps RT = 2 and 4 at 64 registers and spills; a minimum of 2 blocks spills RT = 8, which
+// fits in 91 registers without one (ptxas -v).
+template <int RT>
+__global__ void __launch_bounds__(256, RT <= 4 ? 2 : 0)
+k_affinity_resolve_ranked(const float *__restrict__ fobj, uint64_t n, const float *__restrict__ fnode_g, const uint32_t *__restrict__ nidx_map, uint32_t n_live,
+                          const uint32_t *__restrict__ groups, uint32_t ranks, uint32_t *__restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31, q = lane >> 3, r = lane & 7, seg = lane & ~7u;
+    const uint64_t warp0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    const float4 *fobj4 = reinterpret_cast<const float4 *>(fobj);
+    const float4 *fnode4 = reinterpret_cast<const float4 *>(fnode_g) + r;
+    // one trip ahead, as in k_affinity_resolve: the groups and the row of the next trip are in flight while this trip scores
+    uint64_t base = warp0 * 4;
+    bool mine = base + q < n;
+    uint64_t row = mine ? base + q : n - 1;
+    uint32_t g = kNone;
+    float4 o[4] = {};
+    if (base < n) {
+        if (r < RT) g = __ldg(groups + row * RT + r);
+#pragma unroll
+        for (int k = 0; k < 4; k++) o[k] = __ldg(fobj4 + row * 4 + k);
+    }
+    for (; base < n; base += nwarps * 4) {
+        const uint64_t nbase = base + nwarps * 4;
+        const bool nmine = nbase + q < n;
+        const uint64_t nrow = nmine ? nbase + q : n - 1;
+        uint32_t ng = kNone;
+        float4 no[4] = {};
+        if (nbase < n) {
+            if (r < RT) ng = __ldg(groups + nrow * RT + r);
+#pragma unroll
+            for (int k = 0; k < 4; k++) no[k] = __ldg(fobj4 + nrow * 4 + k);
+        }
+        int key[RT];
+        uint32_t pos[RT];
+#pragma unroll
+        for (int j = 0; j < RT; j++) {
+            const uint32_t gj = __shfl_sync(0xFFFFFFFFu, g, seg | j);
+            const float4 *fn = fnode4 + (size_t)(gj == kNone ? 0u : gj) * 32;
+            float a = 0.f;
+#pragma unroll
+            for (int k = 0; k < 4; k++) {
+                const float4 x = __ldg(fn + k * 8);
+                a = fmaf(o[k].x, x.x, a); a = fmaf(o[k].y, x.y, a); a = fmaf(o[k].z, x.z, a); a = fmaf(o[k].w, x.w, a);
+            }
+            uint32_t p = gj * 8 + r;
+            const bool live = gj != kNone && p < n_live;
+            const uint32_t bits = live ? __float_as_uint(-a) : 0x7F800000u;
+            key[j] = (int)(bits ^ ((uint32_t)((int)bits >> 31) & 0x7FFFFFFFu));
+            pos[j] = live ? p : kNone;
+        }
+        for (uint32_t rank = 0; rank < ranks; rank++) {   // warp-uniform
+            int k = key[0];
+            uint32_t p = pos[0];
+            if (rank) {
+#pragma unroll
+                for (int j = 1; j < RT; j++)
+                    if (key[j] < k || (key[j] == k && pos[j] < p)) { k = key[j]; p = pos[j]; }
+            }
+#pragma unroll
+            for (int d = 4; d >= 1; d >>= 1) {
+                const int ok = __shfl_xor_sync(0xFFFFFFFFu, k, d);
+                const uint32_t op = __shfl_xor_sync(0xFFFFFFFFu, p, d);
+                if (ok < k || (ok == k && op < p)) { k = ok; p = op; }
+            }
+            if (r == 0 && mine) out[row * ranks + rank] = p == kNone ? kNone : __ldg(nidx_map + p);
+            if (p != kNone) {
+#pragma unroll
+                for (int j = 0; j < RT; j++)
+                    if (pos[j] == p) { key[j] = 0x7F800000; pos[j] = kNone; }
+            }
+        }
+        mine = nmine; row = nrow; g = ng;
+#pragma unroll
+        for (int k = 0; k < 4; k++) o[k] = no[k];
+    }
+}
+
 }  // namespace
 
 #define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
@@ -358,6 +564,53 @@ cudaError_t launch_assign_affinity_umma(const Launch &L, const float *d_fobj, ui
         RIO_COUNT_LAUNCH(L);
     }
     return cudaGetLastError();
+}
+
+namespace {
+
+// warpgroups per CTA of k_affinity_wgmma_ranked<NT, RT>: four where the lists fit in 128 registers without spills (ptxas -v)
+constexpr int ranked_warpgroups(int NT, int RT) { return RT <= 4 ? 4 : 2; }
+
+template <int NT, int RT>
+cudaError_t launch_wgmma_ranked(const Launch &L, const WgmmaParams &P, size_t smem) {
+    constexpr int WG = ranked_warpgroups(NT, RT);
+    const uint64_t n_rb = (P.n + kRows - 1) / kRows, n_cta = (n_rb + WG - 1) / WG;
+    const int grid = (int)(n_cta < (uint64_t)L.sm_count ? n_cta : (uint64_t)L.sm_count);
+    cudaError_t err = cudaFuncSetAttribute(k_affinity_wgmma_ranked<NT, RT, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) k_affinity_wgmma_ranked<NT, RT, WG><<<grid, 128 * WG, smem, L.stream>>>(P);
+    return err == cudaSuccess ? cudaGetLastError() : err;
+}
+
+template <int RT>
+cudaError_t launch_ranked_pair(const Launch &L, const WgmmaParams &P, size_t smem, const float *d_fnode_g, const uint32_t *d_nidx_map, uint32_t ranks,
+                               uint32_t *d_out_idx) {
+    const cudaError_t err = P.m_pad <= 64 ? launch_wgmma_ranked<64, RT>(L, P, smem) : launch_wgmma_ranked<128, RT>(L, P, smem);
+    if (err != cudaSuccess) return err;
+    RIO_COUNT_LAUNCH(L);
+    const uint64_t blocks = (P.n + 31) / 32, cap = (uint64_t)L.sm_count * 8;
+    k_affinity_resolve_ranked<RT><<<(int)(blocks < cap ? blocks : cap), 256, 0, L.stream>>>(P.fobj, P.n, d_fnode_g, d_nidx_map, P.n_live, P.out_idx, ranks,
+                                                                                           d_out_idx);
+    RIO_COUNT_LAUNCH(L);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_assign_affinity_umma_ranked(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode_c, const float *d_fnode_g,
+                                               const uint32_t *d_nidx_map, uint32_t n_live, uint32_t m_pad, uint32_t ranks, uint32_t *d_groups,
+                                               uint32_t *d_out_idx) {
+    if (!n) return cudaSuccess;
+    const bool small = m_pad <= 64;
+    if (!n_live || (small && m_pad != 64) || (!small && (m_pad % 256)) || m_pad > affinity_umma_max_nodes() || ranks < 1 || ranks > kMaxRanks)
+        return cudaErrorInvalidValue;
+    const size_t smem = (size_t)3 * m_pad * 32;
+    const WgmmaParams P{d_fobj, n, d_fnode_c, n_live, m_pad, d_groups, nullptr};
+    switch (affinity_ranked_groups(ranks)) {
+        case 1: return launch_ranked_pair<1>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        case 2: return launch_ranked_pair<2>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        case 4: return launch_ranked_pair<4>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        default: return launch_ranked_pair<8>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+    }
 }
 
 }  // namespace rio

@@ -6,6 +6,7 @@
 // The -log2 and the 64-bit weighted score are evaluated once per (object, weight class), not per pair.
 // The kernel is integer-ALU bound (12 B of HBM traffic per object against M pair hashes), see DESIGN.md 5.1.
 #include "kernels.cuh"
+#include "k_affinity_ranked.cuh"
 #include "spec.cuh"
 #include <cstdlib>
 
@@ -408,6 +409,60 @@ k_assign_affinity_generic(const float *__restrict__ fobj, uint64_t n, const floa
     }
 }
 
+// Ranked lists (DESIGN.md 3.9) on the CUDA cores: the node loop and fmaf order of k_assign_affinity / k_assign_affinity_generic,
+// one object per thread, and the RT smallest (cost, j) kept sorted in registers.  A node displaces an entry only with a strictly
+// smaller cost, so equal costs keep the lower j first and the first entry is the unranked kernels' node.  KC = 16 keeps the object
+// row in registers; KC = 0 takes any K at run time.  The first `ranks` (<= RT) entries are written, kNone past the live set.
+template <int KC, int RT>
+__global__ void __launch_bounds__(kAssignThreads)
+k_assign_affinity_ranked(const float *__restrict__ fobj, uint64_t n, const float *__restrict__ fnode, const uint32_t *__restrict__ live,
+                         uint32_t n_total, uint32_t K, uint32_t ranks, uint32_t *__restrict__ out_idx) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        float fo[KC ? KC : 1];
+        if constexpr (KC != 0) {
+            const float4 *row = reinterpret_cast<const float4 *>(fobj + i * KC);
+#pragma unroll
+            for (int k4 = 0; k4 < KC / 4; k4++) {
+                const float4 v = __ldg(row + k4);
+                fo[4 * k4 + 0] = v.x; fo[4 * k4 + 1] = v.y; fo[4 * k4 + 2] = v.z; fo[4 * k4 + 3] = v.w;
+            }
+        }
+        float lc[RT];
+        uint32_t lj[RT];
+#pragma unroll
+        for (int s = 0; s < RT; s++) { lc[s] = 0.f; lj[s] = kNone; }
+        for (uint32_t j = 0; j < n_total; j++) {
+            if (!__ldg(live + j)) continue;
+            float acc = 0.f;
+            if constexpr (KC != 0) {
+                const float4 *nr = reinterpret_cast<const float4 *>(fnode + (size_t)j * KC);
+#pragma unroll
+                for (int k4 = 0; k4 < KC / 4; k4++) {
+                    const float4 v = __ldg(nr + k4);
+                    acc = fmaf(fo[4 * k4 + 0], v.x, acc);
+                    acc = fmaf(fo[4 * k4 + 1], v.y, acc);
+                    acc = fmaf(fo[4 * k4 + 2], v.z, acc);
+                    acc = fmaf(fo[4 * k4 + 3], v.w, acc);
+                }
+            } else {
+                const float *fi = fobj + i * K, *fn = fnode + (size_t)j * K;
+                for (uint32_t k = 0; k < K; k++) acc = fmaf(__ldg(fi + k), __ldg(fn + k), acc);
+            }
+            const float cst = -acc;
+            if (lj[RT - 1] != kNone && !(cst < lc[RT - 1])) continue;
+#pragma unroll
+            for (int s = RT - 1; s > 0; s--) {
+                if (lj[s - 1] == kNone || cst < lc[s - 1]) { lc[s] = lc[s - 1]; lj[s] = lj[s - 1]; }
+                else if (lj[s] == kNone || cst < lc[s]) { lc[s] = cst; lj[s] = j; }
+            }
+            if (lj[0] == kNone || cst < lc[0]) { lc[0] = cst; lj[0] = j; }
+        }
+#pragma unroll
+        for (int s = 0; s < RT; s++)
+            if (s < (int)ranks) out_idx[i * ranks + s] = lj[s];
+    }
+}
+
 
 // Register-only replay of the assign inner loop (same IMAD / IMAD / VIMNMX3 mix, no shared or global
 // memory in the loop): its pair rate is the integer-ALU roofline the assign kernel is reported against.
@@ -587,6 +642,26 @@ void launch_assign_affinity(const Launch &L, const float *d_fobj, uint64_t n, co
         k_assign_affinity_generic<<<grid_for(n, kAssignThreads, L.sm_count, 8), kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K,
                                                                                                        d_out_idx, d_out_cost, d_counters);
     }
+    RIO_COUNT_LAUNCH(L);
+}
+
+template <int KC>
+static void launch_affinity_ranked_k(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode, const uint32_t *d_live, uint32_t n_total,
+                                     uint32_t K, uint32_t ranks, uint32_t *d_out_idx) {
+    const int grid = grid_for(n, kAssignThreads, L.sm_count, 8);
+    switch (affinity_ranked_groups(ranks)) {
+        case 1: k_assign_affinity_ranked<KC, 1><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
+        case 2: k_assign_affinity_ranked<KC, 2><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
+        case 4: k_assign_affinity_ranked<KC, 4><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
+        default: k_assign_affinity_ranked<KC, 8><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
+    }
+}
+
+void launch_assign_affinity_ranked(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode, const uint32_t *d_live, uint32_t n_total,
+                                   uint32_t K, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!n) return;
+    if (K == 16) launch_affinity_ranked_k<16>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx);
+    else launch_affinity_ranked_k<0>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx);
     RIO_COUNT_LAUNCH(L);
 }
 

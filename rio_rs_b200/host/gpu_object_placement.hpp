@@ -121,6 +121,14 @@ class GpuObjectPlacement {
         check(rio_cuda_assign_ranked_batch(e_->h, keys.data(), keys.size(), ranks, out.data()));
         return out;
     }
+    // each object's `ranks` lowest-cost live nodes under the affinity cost (DESIGN.md 3.9); obj_feats is n x K row-major (K of
+    // set_nodes), the result row-major as for assign_ranked
+    std::vector<uint32_t> assign_ranked_affinity(const std::vector<float> &obj_feats, size_t n, uint32_t ranks) const {
+        if (n && obj_feats.size() % n) throw ObjectPlacementError(ObjectPlacementError::Unknown, "obj_feats is not n x K");
+        std::vector<uint32_t> out(n * ranks);
+        check(rio_cuda_assign_ranked_affinity_batch(e_->h, obj_feats.data(), n, ranks, out.data()));
+        return out;
+    }
     std::vector<uint32_t> place_batch(const std::vector<uint64_t> &keys, uint32_t policy, uint32_t self_idx) const {
         std::vector<uint32_t> out(keys.size());
         check(rio_cuda_place_batch(e_->h, keys.data(), keys.size(), policy, self_idx, out.data()));

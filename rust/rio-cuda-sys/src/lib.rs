@@ -75,6 +75,7 @@ extern "C" {
 
     pub fn rio_cuda_assign_batch(h: *mut rio_placement, keys: *const u64, obj_feats: *const f32, n: size_t, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_batch(h: *mut rio_placement, keys: *const u64, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_affinity_batch(h: *mut rio_placement, obj_feats: *const f32, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_place_batch(h: *mut rio_placement, keys: *const u64, n: size_t, policy: u32, self_idx: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_rebalance(h: *mut rio_placement, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_load_counters(h: *mut rio_placement, out: *mut u32, cap: u32) -> rio_status;
@@ -108,6 +109,7 @@ extern "C" {
     pub fn rio_cuda_memcpy_d2h(h: *mut rio_placement, host: *mut c_void, dev: *const c_void, bytes: size_t) -> rio_status;
     pub fn rio_cuda_assign_batch_dev(h: *mut rio_placement, d_keys: *const u64, d_obj_feats: *const f32, n: size_t, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_affinity_batch_dev(h: *mut rio_placement, d_obj_feats: *const f32, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_lookup_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_upsert_batch_dev(h: *mut rio_placement, d_keys: *const u64, d_idx: *const u32, n: size_t) -> rio_status;
 
