@@ -65,10 +65,11 @@ def tensor_cores(p, var, K, n_live):
 @pytest.mark.gpu
 @pytest.mark.parametrize("var", VARIANTS)
 @pytest.mark.parametrize("K,M,n", [(16, 1024, 60000), (16, 37, 5001), (16, 64, 999), (16, 65, 7000), (16, 300, 20000), (16, 2000, 4000), (16, 2400, 3000),
+                                   (16, 66, 3001), (16, 67, 3001), (16, 258, 3001), (16, 259, 3001), (16, 2306, 3001), (16, 2307, 3001),
                                    (8, 64, 3000), (5, 9, 1000)])
 def test_rank_one_is_assign_batch(gp, oracle, K, M, n, var):
     """The shapes of test_gpu_parity.py::test_affinity_cost_argmin; node 3 has weight 0 and node M - 2 is inactive, so neither is
-    live."""
+    live: 64 / 65, 256 / 257 and 2304 / 2305 live nodes sit on either side of a padding step of the tensor-core path."""
     fo, fn = feats(n, M, K)
     w = np.ones(M, dtype=np.uint32)
     w[3] = 0

@@ -1,24 +1,31 @@
 """Builds the C++ conformance harness against the C++ mirror of the trait and runs it (GPU), and checks on CPU that it
-compiles and links against librio_cuda.so."""
+compiles and links against librio_cuda.so.  The harnesses are compiled into a temporary directory, once per process, so the
+suite also runs from a read-only source tree."""
+import atexit
 import os
+import shutil
 import subprocess
+import tempfile
 
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-EXE = os.path.join(ROOT, "tests", "cpp", "backend_conformance")
+_EXES = {}
 
 
 def _build(name="backend_conformance"):
     from rio_rs_b200 import build
 
     build.build()
-    exe = os.path.join(ROOT, "tests", "cpp", name)
-    src = exe + ".cpp"
-    libdir = os.path.join(ROOT, "rio_rs_b200")
-    if not os.path.exists(exe) or os.path.getmtime(exe) < max(os.path.getmtime(src), os.path.getmtime(os.path.join(libdir, "librio_cuda.so"))):
+    if name not in _EXES:
+        d = tempfile.mkdtemp(prefix="rio_cpp_harness_")
+        atexit.register(shutil.rmtree, d, True)
+        exe = os.path.join(d, name)
+        src = os.path.join(ROOT, "tests", "cpp", name + ".cpp")
+        libdir = os.path.join(ROOT, "rio_rs_b200")
         subprocess.check_call(["/usr/bin/g++", "-std=c++17", "-O1", "-o", exe, src, "-L" + libdir, "-lrio_cuda", "-Wl,-rpath," + libdir])
-    return exe
+        _EXES[name] = exe
+    return _EXES[name]
 
 
 def test_cpp_mirror_compiles_and_links():

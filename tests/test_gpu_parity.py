@@ -182,8 +182,10 @@ def test_c2_weighted_rendezvous_1m_x_64(gp, oracle, seed, variant):
 
 
 @pytest.mark.parametrize("variant", ["2", "1"])
-@pytest.mark.parametrize("M,uniform", [(1, True), (2, False), (3, True), (31, False), (33, False), (64, True), (257, False), (1024, False), (1024, True), (1500, False)])
+@pytest.mark.parametrize("M,uniform", [(1, True), (2, False), (3, True), (31, False), (33, False), (64, True), (257, False), (1024, False), (1024, True), (1500, False),
+                                       (8192, False), (8193, False)])
 def test_ragged_node_counts(gp, oracle, M, uniform, variant):
+    """M = 8192 is the largest table staged in one shared-memory chunk, M = 8193 the smallest that takes two."""
     os.environ["RIO_ASSIGN_VARIANT"] = variant
     try:
         p = provider(gp)
@@ -196,10 +198,12 @@ def test_ragged_node_counts(gp, oracle, M, uniform, variant):
 
 
 @pytest.mark.parametrize("variant", ["2", "1"])
-@pytest.mark.parametrize("M,n", [(9000, 6001), (70000, 1501)])
+@pytest.mark.parametrize("M,n", [(9000, 6001), (65535, 1501), (65536, 1501), (70000, 1501)])
 def test_node_tables_larger_than_one_shared_memory_chunk(gp, oracle, M, n, variant):
     """M = 9000: the table is streamed through shared memory in two chunks and the winner is re-hashed from global
-    memory; M = 70000 exceeds the 16-bit positions of k_assign_hrw_v2, so the launcher must route to k_assign_hrw."""
+    memory; M = 70000 exceeds the 16-bit positions of k_assign_hrw_v2, so the launcher must route to k_assign_hrw.
+    M = 65535 is the largest table k_assign_hrw_v2 takes (a class end of 0xFFFF in its packed positions), 65536 the
+    smallest it hands to k_assign_hrw."""
     os.environ["RIO_ASSIGN_VARIANT"] = variant
     try:
         p = provider(gp)
@@ -260,12 +264,15 @@ def test_golden_vectors_on_gpu(gp):
 # ---- solver: affinity cost, 1e-5 relative ------------------------------------------------------------------------
 @pytest.mark.parametrize("variant", ["umma", "ffma"])
 @pytest.mark.parametrize("K,M,n", [(16, 1024, 60000), (16, 37, 5001), (16, 64, 999), (16, 65, 7000), (16, 300, 20000), (16, 2000, 4000), (16, 2400, 3000),
-                                   (8, 64, 3000), (5, 9, 1000)])
+                                   (16, 66, 3001), (16, 67, 3001), (16, 258, 3001), (16, 259, 3001), (16, 2306, 3001), (16, 2307, 3001),
+                                   (16, 2048, 3001), (16, 2049, 3001), (8, 64, 3000), (5, 9, 1000)])
 def test_affinity_cost_argmin(gp, oracle, K, M, n, variant):
     """cost = -dot, argmin (DESIGN.md 3.6).  K == 16 runs on the tensor cores (wgmma, bf16x3 split) unless
     RIO_AFFINITY_VARIANT=ffma or the padded live-node set is larger than the 2304 nodes shared memory holds (M = 2400);
     other K use CUDA cores.  Which path ran is pinned by its launch count: the tensor-core path is two launches
-    (k_affinity_wgmma + k_affinity_resolve), the CUDA-core path one."""
+    (k_affinity_wgmma + k_affinity_resolve), the CUDA-core path one.  Two nodes are not live, so M = 66 / 67, 258 / 259 and
+    2306 / 2307 put 64 / 65, 256 / 257 and 2304 / 2305 live nodes on either side of a padding step (the last pair on either
+    side of the tensor-core limit); M = 2048 / 2049 are one and two node chunks of the CUDA-core K = 16 kernel."""
     rng = np.random.default_rng(11)
     fo = rng.uniform(-1, 1, (n, K)).astype(np.float32)
     fn = np.random.default_rng(13).uniform(-1, 1, (M, K)).astype(np.float32)
