@@ -175,10 +175,25 @@ rio_status  rio_cuda_check_address_batch(rio_placement *h, const uint32_t *addr_
  * service.rs:224-238 / 286-297): RIO_EV_JOIN(idx) moves onto idx exactly the objects that now prefer it;
  * RIO_EV_LEAVE(idx) re-places exactly the objects recorded on idx.  Under RIO_SOLVER_HRW2 every placed key is walked
  * again and the ones whose node changed are rewritten (the state after the call is the fresh assignment over the
- * live set).  out_moved may be NULL. */
+ * live set).  out_moved may be NULL.  A weight decrease under RIO_SOLVER_HRW is applied exactly only by
+ * rio_cuda_rebalance_changes. */
 #define RIO_EV_JOIN  1u
 #define RIO_EV_LEAVE 2u
 rio_status  rio_cuda_rebalance(rio_placement *h, uint32_t event, uint32_t idx, uint64_t *out_moved);
+/* Eager re-placement of the whole directory after a SET of node changes (DESIGN.md 3.10), in one pass.  idx[0..k) are distinct
+ * interned node indices; prev_weight[i] is node idx[i]'s weight before the change if it was live then (active, weight > 0),
+ * else 0.  Apply the changes first (set_nodes / node_upsert / node_set_active); read the prior weights with
+ * rio_cuda_node_state before.  With r = floor((2^32-1)/w) for a live node and 0 otherwise:
+ *   REPLACE    = every interned node not live now, and every changed node live now whose r grew (it lost weight);
+ *   CANDIDATES = every changed node live now that was not live before or whose r shrank (it joined or gained weight);
+ *   a changed node whose r did not change is a no-op.
+ * RIO_SOLVER_HRW: an entry (key, y) with y in REPLACE is re-placed over the current live set (it may stay on y); any other
+ * placed entry goes to the best node of {y} u CANDIDATES under the order of 3.4.  If the directory was the flat assignment
+ * over the previous live set, it is the fresh one over the current live set afterwards.  RIO_SOLVER_HRW2: any k > 0 walks
+ * every placed key again once.  Entries become RIO_NONE when no node is live; k == 0 does nothing.  out_moved (may be NULL)
+ * receives the number of entries whose node changed.  RIO_ERR_UNKNOWN: an index out of range, a duplicate index, NULL arrays
+ * with k > 0; RIO_ERR_UPSTREAM under RIO_SOLVER_HRW when the library was built without the change-set kernels. */
+rio_status  rio_cuda_rebalance_changes(rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved);
 /* Per-node object counts of the directory (out has node_count entries). */
 rio_status  rio_cuda_load_counters(rio_placement *h, uint32_t *out, uint32_t cap);
 
@@ -203,6 +218,10 @@ rio_status  rio_cuda_set_assign_bounded_begin(rio_objset *s, uint64_t n_total, u
 rio_status  rio_cuda_set_assign_bounded_end(rio_objset *s, uint32_t *out_passes);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
+/* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied
+ * again; sets assigned with affinity are not supported).  Objects with no node (RIO_NONE) are re-placed like REPLACE entries.
+ * The counters stay exact.  Also RIO_ERR_UNKNOWN for a set with no assignment yet. */
+rio_status  rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved);
 /* Global (all ranks) per-node counters of the set's current assignment. */
 rio_status  rio_cuda_set_counters(rio_objset *s, uint32_t *out, uint32_t cap);
 rio_status  rio_cuda_set_read(rio_objset *s, uint64_t first, uint64_t n, uint64_t *out_keys, uint32_t *out_idx);

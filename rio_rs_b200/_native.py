@@ -67,6 +67,7 @@ SIGNATURES = {
     "rio_cuda_check_address_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp, u64p]),
     "rio_cuda_place_batch": (C.c_int32, [H, vp, sz, C.c_uint32, C.c_uint32, vp]),
     "rio_cuda_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),
+    "rio_cuda_rebalance_changes": (C.c_int32, [H, vp, vp, sz, u64p]),
     "rio_cuda_load_counters": (C.c_int32, [H, vp, C.c_uint32]),
     "rio_cuda_set_create": (C.c_int32, [H, C.c_uint64, C.POINTER(H)]),
     "rio_cuda_set_destroy": (None, [H]),
@@ -77,6 +78,7 @@ SIGNATURES = {
     "rio_cuda_set_assign_bounded_begin": (C.c_int32, [H, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32]),
     "rio_cuda_set_assign_bounded_end": (C.c_int32, [H, u32p]),
     "rio_cuda_set_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),
+    "rio_cuda_set_rebalance_changes": (C.c_int32, [H, vp, vp, sz, u64p]),
     "rio_cuda_set_counters": (C.c_int32, [H, vp, C.c_uint32]),
     "rio_cuda_set_read": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp, vp]),
     "rio_cuda_set_size": (C.c_int32, [H, u64p]),

@@ -9,6 +9,7 @@
 #include "kernels.cuh"
 #include "k_ranked.cuh"
 #include "k_affinity_ranked.cuh"
+#include "k_changes.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -1426,6 +1427,95 @@ rio_status rio_cuda_rebalance(rio_placement *h, uint32_t event, uint32_t idx, ui
     });
 }
 
+namespace {
+
+// A change set (DESIGN.md 3.10) as the flat-policy kernels see it: one byte per interned node (REPLACE / CANDIDATE / neither) and
+// the list of candidates, uploaded into h->s_misc.  The arguments were checked by check_change_set.
+struct ChangeSetHost {
+    std::vector<uint8_t> bytes;   // n_total flag bytes, padded to 4, then the candidate indices
+    uint32_t n_cand = 0;
+};
+
+void check_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
+    REQUIRE(!k || (idx && prev_weight), "null change-set arrays");
+    const size_t n_total = h->nodes.size();
+    std::vector<uint8_t> seen(n_total, 0);
+    for (size_t i = 0; i < k; i++) {
+        REQUIRE(idx[i] < n_total, "change-set node index out of range");
+        REQUIRE(!seen[idx[i]], "duplicate node index in the change set");
+        seen[idx[i]] = 1;
+    }
+}
+
+ChangeSetHost build_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
+    const uint32_t n_total = (uint32_t)h->nodes.size();
+    const size_t pad = (n_total + 3) & ~(size_t)3;
+    ChangeSetHost cs;
+    cs.bytes.assign(std::max<size_t>(pad, 4), 0);
+    for (uint32_t j = 0; j < n_total; j++) if (!h->nodes[j].live()) cs.bytes[j] = kChgReplace;
+    std::vector<uint32_t> cand;
+    for (size_t i = 0; i < k; i++) {
+        const NodeInfo &ni = h->nodes[idx[i]];
+        if (!ni.live()) continue;   // REPLACE already
+        const uint32_t r_prev = prev_weight[i] ? inv_weight(prev_weight[i]) : 0u, r_now = inv_weight(ni.weight);
+        if (r_prev && r_now > r_prev) cs.bytes[idx[i]] = kChgReplace;                     // lost weight
+        else if (!r_prev || r_now < r_prev) { cs.bytes[idx[i]] = kChgCandidate; cand.push_back(idx[i]); }   // joined or gained weight
+    }
+    cs.n_cand = (uint32_t)cand.size();
+    const size_t o = cs.bytes.size();
+    cs.bytes.resize(o + cand.size() * 4);
+    if (!cand.empty()) memcpy(cs.bytes.data() + o, cand.data(), cand.size() * 4);
+    return cs;
+}
+
+ChangeSetDev upload_change_set(rio_placement *h, const ChangeSetHost &cs) {
+    h->s_misc.ensure(cs.bytes.size(), h->stream);
+    CUDA_TRY(cudaMemcpyAsync(h->s_misc.p, cs.bytes.data(), cs.bytes.size(), cudaMemcpyHostToDevice, h->stream));
+    const uint8_t *d = h->s_misc.as<uint8_t>();
+    return ChangeSetDev{d, reinterpret_cast<const uint32_t *>(d + cs.bytes.size() - (size_t)cs.n_cand * 4), cs.n_cand};
+}
+
+void require_change_kernels() {
+    if (!launch_dir_rebalance_changes || !launch_dir_scatter_changes || !launch_rebalance_changes || !launch_count_changed)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no change-set kernels (k_directory.cu without them is linked)"};
+}
+
+}  // namespace
+
+rio_status rio_cuda_rebalance_changes(rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_change_set(h, idx, prev_weight, k);
+        uint64_t moved = 0;
+        if (k) {
+            ensure_tab(h);
+            zero_scalar(h, S_MOVED);
+            if (h->solver == RIO_SOLVER_HRW2) {   // one re-walk of every placed key, whatever the change set holds
+                launch_dir_reassign_trie(h->L(), h->dir, h->tabs.trie, h->d_scalars + S_MOVED);
+            } else {
+                require_change_kernels();
+                const ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
+                const ChangeSetDev dcs = upload_change_set(h, cs);
+                // every claimed key could be an R1 entry (all nodes left): the lists are sized for that, grow-only
+                const uint64_t max_r1 = std::max<uint64_t>(h->dir_keys + h->dir_keys_pending, 1);
+                h->s_slots.ensure(max_r1 * 8, h->stream);
+                h->s_keys2.ensure(max_r1 * 8, h->stream);
+                zero_scalar(h, S_NSEL);
+                launch_dir_rebalance_changes(h->L(), h->dir, h->tabs.tab, dcs, h->s_slots.as<uint64_t>(), h->s_keys2.as<uint64_t>(), h->d_scalars + S_NSEL,
+                                             h->d_scalars + S_MOVED);
+                const uint64_t n_r1 = read_scalar(h, S_NSEL);
+                if (n_r1) {
+                    h->s_idx2.ensure(n_r1 * 4, h->stream);
+                    launch_assign_hrw(h->L(), h->s_keys2.as<uint64_t>(), n_r1, h->tabs.tab, h->s_idx2.as<uint32_t>(), nullptr, nullptr, 0);
+                    launch_dir_scatter_changes(h->L(), h->dir, h->s_slots.as<uint64_t>(), h->s_idx2.as<uint32_t>(), n_r1, h->d_scalars + S_MOVED);
+                }
+            }
+            moved = read_scalar(h, S_MOVED);
+        }
+        if (out_moved) *out_moved = moved;
+    });
+}
+
 // ---- resident object sets --------------------------------------------------------------------------------------------
 rio_status rio_cuda_set_create(rio_placement *h, uint64_t capacity, rio_objset **out) {
     if (!h || !out) { g_last_error = "null argument"; return RIO_ERR_UNKNOWN; }
@@ -1581,6 +1671,41 @@ rio_status rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, u
             moved = read_scalar(h, S_NSEL);
             CUDA_TRY(cudaMemsetAsync(s->counters.as<uint32_t>() + idx, 0, 4, h->stream));
             if (moved) run_assign(h, RIO_SOLVER_HRW, h->tabs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->sel.as<uint32_t>(), moved);
+        }
+        if (out_moved) *out_moved = moved;
+    });
+}
+
+rio_status rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        check_change_set(h, idx, prev_weight, k);
+        REQUIRE(s->assigned, "set has no assignment yet");
+        uint64_t moved = 0;
+        if (k) {
+            ensure_tab(h);
+            set_ensure_counters(s);
+            zero_scalar(h, S_MOVED);
+            if (h->solver == RIO_SOLVER_HRW2) {   // one re-walk of every key, counters rebuilt, as rio_cuda_set_rebalance does
+                CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+                launch_reassign_trie(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), h->tabs.tab.n_total,
+                                     h->d_scalars + S_MOVED);
+            } else {
+                require_change_kernels();
+                const ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
+                const ChangeSetDev dcs = upload_change_set(h, cs);
+                h->s_idx2.ensure(std::max<uint64_t>(s->n, 1) * 4, h->stream);   // old node of each selected object
+                zero_scalar(h, S_NSEL);
+                launch_rebalance_changes(h->L(), s->keys.as<uint64_t>(), s->idx.as<uint32_t>(), s->n, h->tabs.tab, dcs, s->counters.as<uint32_t>(),
+                                         s->sel.as<uint32_t>(), h->s_idx2.as<uint32_t>(), h->d_scalars + S_NSEL, h->d_scalars + S_MOVED);
+                const uint64_t n_sel = read_scalar(h, S_NSEL);
+                if (n_sel) {
+                    run_assign(h, RIO_SOLVER_HRW, h->tabs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel);
+                    launch_count_changed(h->L(), s->idx.as<uint32_t>(), s->sel.as<uint32_t>(), h->s_idx2.as<uint32_t>(), n_sel, h->d_scalars + S_MOVED);
+                }
+            }
+            moved = read_scalar(h, S_MOVED);
         }
         if (out_moved) *out_moved = moved;
     });

@@ -2,6 +2,7 @@
 // streaming rebalance kernels.  Integer/byte work, HBM-bound: one 16-byte slot per probe (a 32-byte sector holds
 // two slots), 128-bit loads on the scans, warp-aggregated counters.
 #include "kernels.cuh"
+#include "k_changes.cuh"
 #include "spec.cuh"
 #include "bounded_tail.cuh"
 
@@ -203,6 +204,16 @@ k_dir_count(DirDev dir, unsigned long long *placed, uint32_t *counters, uint32_t
 // incumbent that is not live (recorded on an inactive / zero-weight / never-live address: update() may record anything) is
 // re-placed by the full rendezvous over the live table, exactly what a fresh assignment would do -- not handed to the joiner.
 __device__ uint32_t hrw_scalar(uint64_t key, const NodeTabDev &tab);
+// Does node jn (pair hash un, factor rn) beat node jc (uc, rc) under the spec order?  Cheap bracket first: E(u) lies in
+// [clz(u) << 26, (clz(u)+1) << 26], so most comparisons (the challenger wins only ~w/W of the time) are decided without
+// evaluating the log polynomial at all.
+__device__ __forceinline__ bool challenger_wins(uint32_t un, uint32_t rn, uint32_t jn, uint32_t uc, uint32_t rc, uint32_t jc) {
+    const uint32_t ln = clz_u32(un), lc = clz_u32(uc);
+    if ((uint64_t)(ln << 26) * rn > (uint64_t)((lc + 1u) << 26) * rc) return false;
+    const uint64_t sn = (uint64_t)elog(un) * rn;
+    const uint64_t sc = (uint64_t)elog(uc) * rc;
+    return cand_better(sn, un, jn, sc, uc, jc);
+}
 __device__ __forceinline__ bool join_wins(uint64_t key, uint32_t cur, uint32_t new_idx, const uint4 nn, const uint4 *by_idx, bool *incumbent_dead) {
     const ObjHash o = obj_hash(key);
     const uint32_t un = pair_hash(o, nn.x, nn.z, nn.w);
@@ -210,13 +221,7 @@ __device__ __forceinline__ bool join_wins(uint64_t key, uint32_t cur, uint32_t n
     *incumbent_dead = c.y == 0;
     if (c.y == 0) return false;
     const uint32_t uc = pair_hash(o, c.x, c.z, c.w);
-    // cheap bracket first: E(u) lies in [clz(u) << 26, (clz(u)+1) << 26], so most comparisons (the new node wins only
-    // ~w/W of the time) are decided without evaluating the log polynomial at all
-    const uint32_t ln = clz_u32(un), lc = clz_u32(uc);
-    if ((uint64_t)(ln << 26) * nn.y > (uint64_t)((lc + 1u) << 26) * c.y) return false;
-    const uint64_t sn = (uint64_t)elog(un) * nn.y;
-    const uint64_t sc = (uint64_t)elog(uc) * c.y;
-    return cand_better(sn, un, new_idx, sc, uc, cur);
+    return challenger_wins(un, nn.y, new_idx, uc, c.y, cur);
 }
 
 // The incumbent's node record is a random 16-byte gather: from L1 that costs one wavefront per distinct line (up to 32 per
@@ -388,6 +393,191 @@ k_dir_rebalance_leave(DirDev dir, NodeTabDev tab, uint32_t gone, unsigned long l
         }
         warp_add(moved, mv);
     }
+}
+
+// ---- change set (DESIGN.md 3.10): R1 entries (incumbent in REPLACE) are collected and re-placed by the grid kernel;
+// an R2 entry goes to the best of {incumbent} u CANDIDATES, one pair hash each, decided in place.
+// Shared-memory layout when staged: [n_total x uint4 by-index records][n_cand x u32 candidates][n_total flag bytes].
+template <bool SMEM>
+__device__ __forceinline__ ChangeSetDev stage_changes(const ChangeSetDev &cs, uint32_t n_total) {
+    extern __shared__ __align__(16) unsigned char smem_dir[];
+    if (!SMEM) return cs;
+    uint32_t *c = reinterpret_cast<uint32_t *>(smem_dir + (size_t)n_total * 16);
+    uint8_t *f = reinterpret_cast<uint8_t *>(c + cs.n_cand);
+    for (uint32_t j = threadIdx.x; j < cs.n_cand; j += blockDim.x) c[j] = __ldg(cs.cand + j);
+    for (uint32_t j = threadIdx.x; j < n_total; j += blockDim.x) f[j] = __ldg(cs.flag + j);
+    return ChangeSetDev{f, c, cs.n_cand};   // visible after the __syncthreads of stage_by_idx
+}
+
+__device__ __forceinline__ uint32_t change_target(uint64_t key, uint32_t cur, const uint4 *by_idx, const ChangeSetDev &cs) {
+    const ObjHash o = obj_hash(key);
+    const uint4 c = by_idx[cur];
+    uint32_t best = cur, bu = pair_hash(o, c.x, c.z, c.w), br = c.y;
+    for (uint32_t q = 0; q < cs.n_cand; q++) {
+        const uint32_t j = cs.cand[q];
+        const uint4 r = by_idx[j];
+        const uint32_t u = pair_hash(o, r.x, r.z, r.w);
+        if (challenger_wins(u, r.y, j, bu, br, best)) { best = j; bu = u; br = r.y; }
+    }
+    return best;
+}
+
+// Every lane of the warp calls this with its number of items; returns the position of the lane's first item in a list whose
+// length is *n (one atomic per warp).
+__device__ __forceinline__ unsigned long long warp_reserve(unsigned long long *n, uint32_t mine) {
+    const unsigned lane = threadIdx.x & 31;
+    uint32_t pre = mine;   // inclusive warp prefix sum
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, pre, o); if (lane >= (unsigned)o) pre += t; }
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, pre, 31);
+    unsigned long long b = 0;
+    if (lane == 0 && total) b = atomicAdd(n, (unsigned long long)total);
+    return __shfl_sync(0xFFFFFFFFu, b, 0) + (pre - mine);
+}
+
+// Directory, 16 B/slot stream: four independent 128-bit slot loads per thread per trip.  The trip loop is warp-uniform (the
+// capacity is a power of two >= 1024), so the R1 append can ballot.
+template <bool SMEM>
+__global__ void __launch_bounds__(256)
+k_dir_rebalance_changes(DirDev dir, NodeTabDev tab, ChangeSetDev cs_in, uint64_t *__restrict__ r1_slot, uint64_t *__restrict__ r1_key,
+                        unsigned long long *nr1, unsigned long long *moved) {
+    const ChangeSetDev cs = stage_changes<SMEM>(cs_in, tab.n_total);
+    const uint4 *by_idx = stage_by_idx<SMEM>(tab);
+    const uint4 *slots = reinterpret_cast<const uint4 *>(dir.slots);
+    const uint64_t cap = dir.mask + 1, stride = (uint64_t)gridDim.x * blockDim.x;
+    unsigned long long n_moved = 0;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < cap; i0 += stride * 4) {
+        uint4 v[4];
+#pragma unroll
+        for (int e = 0; e < 4; e++) { const uint64_t i = i0 + e * stride; v[e] = i < cap ? slots[i] : make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, kNone, 0); }
+        uint32_t r1 = 0;   // bit e: slot e goes to the R1 list
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const unsigned long long key = ((unsigned long long)v[e].y << 32) | v[e].x;
+            if (key == kEmptyKey || v[e].z >= tab.n_total) continue;
+            if (cs.flag[v[e].z] & kChgReplace) { r1 |= 1u << e; continue; }
+            const uint32_t to = change_target(key, v[e].z, by_idx, cs);
+            if (to != v[e].z) { reinterpret_cast<uint32_t *>(&dir.slots[i0 + e * stride].val)[0] = to; n_moved++; }
+        }
+        if (__ballot_sync(0xFFFFFFFFu, r1 != 0) == 0) continue;
+        unsigned long long b = warp_reserve(nr1, __popc(r1));
+#pragma unroll
+        for (int e = 0; e < 4; e++)
+            if (r1 >> e & 1) { r1_slot[b] = i0 + e * stride; r1_key[b] = ((unsigned long long)v[e].y << 32) | v[e].x; b++; }
+    }
+    warp_flush(moved, n_moved);
+}
+
+__global__ void __launch_bounds__(256)
+k_dir_scatter_changes(DirDev dir, const uint64_t *__restrict__ r1_slot, const uint32_t *__restrict__ to, uint64_t n, unsigned long long *moved) {
+    unsigned long long n_moved = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        uint32_t *node = reinterpret_cast<uint32_t *>(&dir.slots[__ldg(r1_slot + i)].val);
+        const uint32_t t = __ldg(to + i);
+        if (t != *node) { *node = t; n_moved++; }
+    }
+    warp_flush(moved, n_moved);
+}
+
+// The counters of REPLACE nodes: every object on such a node is selected and re-placed, and the re-placement adds its result.
+__device__ __forceinline__ void zero_replace_counters(const ChangeSetDev &cs, uint32_t n_total, uint32_t *counters) {
+    if (!counters) return;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < n_total; j += gridDim.x * blockDim.x)
+        if (__ldg(cs.flag + j) & kChgReplace) counters[j] = 0;
+}
+
+// Dense set, 12 B/object: each thread takes 4 consecutive objects per trip (two 128-bit key loads, one 128-bit index load).
+// An object that is not placed (RIO_NONE, or an index past the table) is selected too: the fresh assignment places it.
+template <bool SMEM>
+__global__ void __launch_bounds__(256)
+k_rebalance_changes(const uint64_t *__restrict__ keys, uint32_t *__restrict__ idx, uint64_t n, NodeTabDev tab, ChangeSetDev cs_in,
+                    uint32_t *__restrict__ counters, uint32_t *__restrict__ sel, uint32_t *__restrict__ sel_old, unsigned long long *nsel,
+                    unsigned long long *moved) {
+    zero_replace_counters(cs_in, tab.n_total, counters);
+    const ChangeSetDev cs = stage_changes<SMEM>(cs_in, tab.n_total);
+    const uint4 *by_idx = stage_by_idx<SMEM>(tab);
+    const uint64_t n_quads = (n + kJoinOpt - 1) / kJoinOpt, stride = (uint64_t)gridDim.x * blockDim.x;
+    unsigned long long n_moved = 0;
+    for (uint64_t qb = (uint64_t)blockIdx.x * blockDim.x; qb < n_quads; qb += stride) {   // block-uniform trips
+        const uint64_t q = qb + threadIdx.x, f = q * kJoinOpt;
+        uint64_t k[4] = {0, 0, 0, 0};
+        uint32_t c[4] = {kNone, kNone, kNone, kNone};
+        if (q < n_quads && f + 3 < n) {
+            const ulonglong2 k0 = __ldg(reinterpret_cast<const ulonglong2 *>(keys + f)), k1 = __ldg(reinterpret_cast<const ulonglong2 *>(keys + f + 2));
+            const uint4 c4 = *reinterpret_cast<const uint4 *>(idx + f);
+            k[0] = k0.x; k[1] = k0.y; k[2] = k1.x; k[3] = k1.y;
+            c[0] = c4.x; c[1] = c4.y; c[2] = c4.z; c[3] = c4.w;
+        } else if (q < n_quads) {
+#pragma unroll
+            for (int e = 0; e < 4; e++) if (f + e < n) { k[e] = __ldg(keys + f + e); c[e] = idx[f + e]; }
+        }
+        uint32_t r1 = 0;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            if (q >= n_quads || f + e >= n) continue;
+            if (c[e] >= tab.n_total || (cs.flag[c[e]] & kChgReplace)) { r1 |= 1u << e; continue; }
+            const uint32_t to = change_target(k[e], c[e], by_idx, cs);
+            if (to != c[e]) {
+                idx[f + e] = to;
+                n_moved++;
+                if (counters) { atomicSub(&counters[c[e]], 1u); atomicAdd(&counters[to], 1u); }
+            }
+        }
+        if (__ballot_sync(0xFFFFFFFFu, r1 != 0) == 0) continue;
+        unsigned long long b = warp_reserve(nsel, __popc(r1));
+#pragma unroll
+        for (int e = 0; e < 4; e++)
+            if (r1 >> e & 1) { sel[b] = (uint32_t)(f + e); sel_old[b] = c[e]; b++; }
+    }
+    warp_flush(moved, n_moved);
+}
+
+// No candidates: no entry takes the R2 branch, so only the selection is left -- a 4 B/object scan of idx, the multi-node form of
+// k_select_on_node (4 x 4 objects per thread per trip).
+__global__ void __launch_bounds__(256)
+k_select_flagged(const uint32_t *__restrict__ idx, uint64_t n, ChangeSetDev cs, uint32_t n_total, uint32_t *__restrict__ counters,
+                 uint32_t *__restrict__ sel, uint32_t *__restrict__ sel_old, unsigned long long *nsel) {
+    zero_replace_counters(cs, n_total, counters);
+    const uint64_t n4 = (n + 3) / 4, stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t base = (uint64_t)blockIdx.x * blockDim.x; base < n4; base += stride * 4) {
+        uint4 x[4];
+        uint32_t valid[4];   // bit q: object 4v+q exists
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const uint64_t v = base + e * stride + threadIdx.x;
+            valid[e] = v < n4 ? (4 * v + 3 < n ? 15u : (1u << (n - 4 * v)) - 1u) : 0u;
+            if (valid[e] == 15u) x[e] = __ldg(reinterpret_cast<const uint4 *>(idx) + v);
+            else if (valid[e]) { x[e].x = __ldg(idx + 4 * v); x[e].y = 4 * v + 1 < n ? __ldg(idx + 4 * v + 1) : 0; x[e].z = 4 * v + 2 < n ? __ldg(idx + 4 * v + 2) : 0; x[e].w = 0; }
+        }
+        uint32_t hits4[4];
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            hits4[e] = 0;
+            if (!valid[e]) continue;
+            const uint32_t xs[4] = {x[e].x, x[e].y, x[e].z, x[e].w};
+#pragma unroll
+            for (int qq = 0; qq < 4; qq++)
+                if ((valid[e] >> qq & 1) && (xs[qq] >= n_total || (cs.flag[xs[qq]] & kChgReplace))) hits4[e] |= 1u << qq;
+        }
+        if (__ballot_sync(0xFFFFFFFFu, (hits4[0] | hits4[1] | hits4[2] | hits4[3]) != 0) == 0) continue;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const uint64_t v = base + e * stride + threadIdx.x;
+            if (__ballot_sync(0xFFFFFFFFu, hits4[e] != 0) == 0) continue;
+            unsigned long long b = warp_reserve(nsel, __popc(hits4[e]));
+            const uint32_t xs[4] = {x[e].x, x[e].y, x[e].z, x[e].w};
+#pragma unroll
+            for (int qq = 0; qq < 4; qq++) if (hits4[e] >> qq & 1) { sel[b] = (uint32_t)(4 * v + qq); sel_old[b] = xs[qq]; b++; }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+k_count_changed(const uint32_t *__restrict__ idx, const uint32_t *__restrict__ sel, const uint32_t *__restrict__ sel_old, uint64_t n, unsigned long long *moved) {
+    unsigned long long n_moved = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+        n_moved += __ldg(idx + __ldg(sel + i)) != __ldg(sel_old + i);
+    warp_flush(moved, n_moved);
 }
 
 // bounded-load rounds: spill selection (DESIGN.md 3.5)
@@ -588,6 +778,54 @@ void launch_rebalance_join(const Launch &L, const uint64_t *d_keys, uint32_t *d_
     } else {
         k_rebalance_join<false><<<grid, 256, 0, L.stream>>>(d_keys, d_idx, n, tab, new_idx, d_counters, d_moved);
     }
+    RIO_COUNT_LAUNCH(L);
+}
+// The change-set passes stage the by-index records, the candidate list and the flag table when the node table fits as JOIN's
+// does (<= 6144 interned nodes: at most 96 + 24 + 6 KB); otherwise every read goes to global memory.
+static size_t changes_smem(const NodeTabDev &tab, const ChangeSetDev &cs) {
+    return tab.n_total <= 6144 ? (size_t)tab.n_total * 17 + (size_t)cs.n_cand * 4 : 0;
+}
+static int changes_ctas_per_sm(size_t smem) { return smem ? (int)std::max<size_t>(1, std::min<size_t>(8, (200u << 10) / smem)) : 8; }
+constexpr int kChangesMaxSmem = 6144 * 21;
+
+void launch_dir_rebalance_changes(const Launch &L, const DirDev &dir, const NodeTabDev &tab, const ChangeSetDev &cs, uint64_t *d_r1_slot, uint64_t *d_r1_key,
+                                  unsigned long long *d_nr1, unsigned long long *d_moved) {
+    const size_t smem = changes_smem(tab, cs);
+    const int grid = grid_for((dir.mask + 1 + 3) / 4, 256, L.sm_count, changes_ctas_per_sm(smem));
+    if (smem) {
+        cudaFuncSetAttribute(k_dir_rebalance_changes<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChangesMaxSmem);
+        k_dir_rebalance_changes<true><<<grid, 256, smem, L.stream>>>(dir, tab, cs, d_r1_slot, d_r1_key, d_nr1, d_moved);
+    } else {
+        k_dir_rebalance_changes<false><<<grid, 256, 0, L.stream>>>(dir, tab, cs, d_r1_slot, d_r1_key, d_nr1, d_moved);
+    }
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_dir_scatter_changes(const Launch &L, const DirDev &dir, const uint64_t *d_r1_slot, const uint32_t *d_to, uint64_t n, unsigned long long *d_moved) {
+    if (!n) return;
+    k_dir_scatter_changes<<<grid_for(n, 256, L.sm_count, 8), 256, 0, L.stream>>>(dir, d_r1_slot, d_to, n, d_moved);
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_rebalance_changes(const Launch &L, const uint64_t *d_keys, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab, const ChangeSetDev &cs,
+                              uint32_t *d_counters, uint32_t *d_sel, uint32_t *d_sel_old, unsigned long long *d_nsel, unsigned long long *d_moved) {
+    if (!n) return;
+    if (!cs.n_cand) {
+        k_select_flagged<<<grid_for((n + 15) / 16, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_idx, n, cs, tab.n_total, d_counters, d_sel, d_sel_old, d_nsel);
+        RIO_COUNT_LAUNCH(L);
+        return;
+    }
+    const size_t smem = changes_smem(tab, cs);
+    const int grid = grid_for((n + kJoinOpt - 1) / kJoinOpt, 256, L.sm_count, changes_ctas_per_sm(smem));
+    if (smem) {
+        cudaFuncSetAttribute(k_rebalance_changes<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChangesMaxSmem);
+        k_rebalance_changes<true><<<grid, 256, smem, L.stream>>>(d_keys, d_idx, n, tab, cs, d_counters, d_sel, d_sel_old, d_nsel, d_moved);
+    } else {
+        k_rebalance_changes<false><<<grid, 256, 0, L.stream>>>(d_keys, d_idx, n, tab, cs, d_counters, d_sel, d_sel_old, d_nsel, d_moved);
+    }
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_count_changed(const Launch &L, const uint32_t *d_idx, const uint32_t *d_sel, const uint32_t *d_sel_old, uint64_t n_sel, unsigned long long *d_moved) {
+    if (!n_sel) return;
+    k_count_changed<<<grid_for(n_sel, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_idx, d_sel, d_sel_old, n_sel, d_moved);
     RIO_COUNT_LAUNCH(L);
 }
 void launch_select_on_node(const Launch &L, const uint32_t *d_idx, uint64_t n, uint32_t node, uint32_t *d_sel, unsigned long long *d_nsel) {

@@ -135,6 +135,14 @@ class GpuObjectPlacement {
         return out;
     }
     uint64_t rebalance(uint32_t event, uint32_t idx) const { uint64_t m = 0; check(rio_cuda_rebalance(e_->h, event, idx, &m)); return m; }
+    // one pass for a set of node changes (DESIGN.md 3.10): {node index, its weight before the change if it was live then, else 0}
+    uint64_t rebalance_changes(const std::vector<std::pair<uint32_t, uint32_t>> &changes) const {
+        std::vector<uint32_t> idx, prev;
+        for (const auto &c : changes) { idx.push_back(c.first); prev.push_back(c.second); }
+        uint64_t m = 0;
+        check(rio_cuda_rebalance_changes(e_->h, idx.data(), prev.data(), idx.size(), &m));
+        return m;
+    }
 };
 
 }  // namespace rio_rs

@@ -76,6 +76,14 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def _change_set(idx, prev_weight):
+    idx = np.ascontiguousarray(idx, dtype=np.uint32)
+    prev = np.ascontiguousarray(prev_weight, dtype=np.uint32)
+    if idx.shape != prev.shape or idx.ndim != 1:
+        raise Unknown("idx and prev_weight must be 1-D arrays of one length")
+    return idx, prev
+
+
 def object_key(type_, id_):
     t, i = type_.encode(), id_.encode()
     return N.lib().rio_cuda_object_key(t, len(t), i, len(i))
@@ -196,6 +204,13 @@ class GpuObjectPlacement:
         a, b = C.c_uint32(0), C.c_uint32(0)
         self._ck(self.L.rio_cuda_node_count(self.h, C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def node_state(self, idx):
+        """(active, weight, malformed) of an interned node.  Read the weights of the nodes a change set is about before applying it:
+        rebalance_changes takes them as prev_weight (0 for a node that was not live)."""
+        a, w, m = C.c_int32(0), C.c_uint32(0), C.c_int32(0)
+        self._ck(self.L.rio_cuda_node_state(self.h, idx, C.byref(a), C.byref(w), C.byref(m)))
+        return bool(a.value), w.value, bool(m.value)
 
     # ---- batched directory ------------------------------------------------------------------------------
     def hash_ids(self, ids):
@@ -327,6 +342,14 @@ class GpuObjectPlacement:
     def rebalance(self, event, idx):
         m = C.c_uint64(0)
         self._ck(self.L.rio_cuda_rebalance(self.h, N.EV_JOIN if event == "join" else N.EV_LEAVE, idx, C.byref(m)))
+        return m.value
+
+    def rebalance_changes(self, idx, prev_weight):
+        """Eager re-placement of the directory after a set of node changes, in one pass (DESIGN.md 3.10): idx are distinct node
+        indices, prev_weight[i] the weight of idx[i] before the change if it was live then, else 0.  Returns the number moved."""
+        idx, prev = _change_set(idx, prev_weight)
+        m = C.c_uint64(0)
+        self._ck(self.L.rio_cuda_rebalance_changes(self.h, _ptr(idx), _ptr(prev), len(idx), C.byref(m)))
         return m.value
 
     # ---- misc --------------------------------------------------------------------------------------------
@@ -516,6 +539,13 @@ class ObjectSet:
     def rebalance(self, event, idx):
         m = C.c_uint64(0)
         self._ck(self.L.rio_cuda_set_rebalance(self.s, N.EV_JOIN if event == "join" else N.EV_LEAVE, idx, C.byref(m)))
+        return m.value
+
+    def rebalance_changes(self, idx, prev_weight):
+        """GpuObjectPlacement.rebalance_changes for this set (plain policy); the counters stay exact."""
+        idx, prev = _change_set(idx, prev_weight)
+        m = C.c_uint64(0)
+        self._ck(self.L.rio_cuda_set_rebalance_changes(self.s, _ptr(idx), _ptr(prev), len(idx), C.byref(m)))
         return m.value
 
     def counters(self):

@@ -164,6 +164,15 @@ impl GpuObjectPlacement {
         check(self.h(), unsafe { sys::rio_cuda_rebalance(self.h(), if join { sys::RIO_EV_JOIN } else { sys::RIO_EV_LEAVE }, node_idx, &mut moved) })?;
         Ok(moved)
     }
+    /// Eager re-placement after a set of node changes, in one pass (DESIGN.md 3.10): each change is (node index, its weight before
+    /// the change if it was live then, else 0), read with `rio_cuda_node_state` before the changes were applied.
+    pub fn rebalance_changes(&self, changes: &[(u32 /*idx*/, u32 /*prev_weight*/)]) -> Result<u64, ObjectPlacementError> {
+        let idx: Vec<u32> = changes.iter().map(|c| c.0).collect();
+        let prev: Vec<u32> = changes.iter().map(|c| c.1).collect();
+        let mut moved = 0u64;
+        check(self.h(), unsafe { sys::rio_cuda_rebalance_changes(self.h(), idx.as_ptr(), prev.as_ptr(), idx.len(), &mut moved) })?;
+        Ok(moved)
+    }
     /// Solver policy of the handle: `hierarchical = false` is the flat weighted rendezvous (minimal movement, M pair hashes per
     /// object), `true` is HRW2 (DESIGN.md 3.8: ~log2 M contests per object, ~(1 + log2(M)/2)x the minimal movement).
     pub fn set_solver(&self, hierarchical: bool, trie_bits: u32) -> Result<(), ObjectPlacementError> {

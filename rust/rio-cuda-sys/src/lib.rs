@@ -78,6 +78,7 @@ extern "C" {
     pub fn rio_cuda_assign_ranked_affinity_batch(h: *mut rio_placement, obj_feats: *const f32, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_place_batch(h: *mut rio_placement, keys: *const u64, n: size_t, policy: u32, self_idx: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_rebalance(h: *mut rio_placement, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
+    pub fn rio_cuda_rebalance_changes(h: *mut rio_placement, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_load_counters(h: *mut rio_placement, out: *mut u32, cap: u32) -> rio_status;
 
     pub fn rio_cuda_set_create(h: *mut rio_placement, capacity: u64, out: *mut *mut rio_objset) -> rio_status;
@@ -89,6 +90,7 @@ extern "C" {
     pub fn rio_cuda_set_assign_bounded_begin(s: *mut rio_objset, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32) -> rio_status;
     pub fn rio_cuda_set_assign_bounded_end(s: *mut rio_objset, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_rebalance(s: *mut rio_objset, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
+    pub fn rio_cuda_set_rebalance_changes(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_counters(s: *mut rio_objset, out: *mut u32, cap: u32) -> rio_status;
     pub fn rio_cuda_set_read(s: *mut rio_objset, first: u64, n: u64, out_keys: *mut u64, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_set_size(s: *mut rio_objset, out_n: *mut u64) -> rio_status;
