@@ -222,6 +222,24 @@ rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, 
  * again; sets assigned with affinity are not supported).  Objects with no node (RIO_NONE) are re-placed like REPLACE entries.
  * The counters stay exact.  Also RIO_ERR_UNKNOWN for a set with no assignment yet. */
 rio_status  rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved);
+/* Ranked resident sets (DESIGN.md 3.11).  rio_cuda_set_assign_ranked computes each key's first `ranks` nodes under the handle's
+ * policy (as rio_cuda_assign_ranked_batch does), keeps them in the set (capacity x ranks x 4 bytes, grow-only, freed by
+ * set_destroy), sets the set's assignment to column 0 and rebuilds the counters from it; the lists record the solver and trie_bits.
+ * rio_cuda_set_read_ranked copies rows [first, first+n) row-major into out (n x ranks entries).
+ * rio_cuda_set_rebalance_changes_ranked takes a change set as rio_cuda_set_rebalance_changes does and leaves every list equal to
+ * the fresh ranked list over the current live set: under RIO_SOLVER_HRW a list with a member in REPLACE (or past the node table) is
+ * recomputed, any other becomes the first `ranks` nodes of itself u CANDIDATES; under RIO_SOLVER_HRW2 any k > 0 walks every list
+ * again.  Only changed rows are written; column 0 stays the set's assignment and the counters stay exact.  out_moved (may be NULL)
+ * receives the number of objects whose rank 1 changed, out_changed (may be NULL) the number whose list changed at any rank.
+ * RIO_ERR_UNKNOWN: ranks outside [1, RIO_MAX_RANKS], n x ranks overflowing, a read outside the set, NULL buffers, the argument
+ * errors of rio_cuda_set_rebalance_changes, a set holding no lists, or a change set under another solver or trie_bits than the
+ * lists were computed with.  RIO_ERR_UPSTREAM when the library was built without the ranked-set kernels.  Every call that rewrites
+ * the set's assignment otherwise (set_load_keys, set_synth_keys, set_assign, set_assign_bounded(_begin), set_rebalance,
+ * set_rebalance_changes) drops the lists. */
+rio_status  rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks);
+rio_status  rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out);
+rio_status  rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved,
+                                                  uint64_t *out_changed);
 /* Global (all ranks) per-node counters of the set's current assignment. */
 rio_status  rio_cuda_set_counters(rio_objset *s, uint32_t *out, uint32_t cap);
 rio_status  rio_cuda_set_read(rio_objset *s, uint64_t first, uint64_t n, uint64_t *out_keys, uint32_t *out_idx);

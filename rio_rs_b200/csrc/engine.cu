@@ -10,6 +10,7 @@
 #include "k_ranked.cuh"
 #include "k_affinity_ranked.cuh"
 #include "k_changes.cuh"
+#include "k_ranked_changes.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -130,7 +131,8 @@ struct TabBufs {
 };
 
 // device scalars (one small allocation): [0]=nsel [1]=moved/removed [2]=new keys (cumulative) [3]=placed ; u32 error at [8]
-enum { S_NSEL = 0, S_MOVED = 1, S_NEWKEYS = 2, S_PLACED = 3, S_FLAGS = 4 /* host-only: {any over, open nodes} written by k_exchange_check */, S_COUNT = 8 };
+enum { S_NSEL = 0, S_MOVED = 1, S_NEWKEYS = 2, S_PLACED = 3, S_FLAGS = 4 /* host-only: {any over, open nodes} written by k_exchange_check */, S_CHANGED = 5,
+       S_COUNT = 8 };
 
 // Device + host state of one bounded-load call in flight (DESIGN.md 3.5): capacities, global counters, thresholds, closed set,
 // the fused tail's ticket, and three words of mapped pinned memory the capacity check reports into.  Every resident set owns
@@ -217,6 +219,11 @@ struct rio_objset {
     bool alt_zero = false;     // counters_alt is known to be all zero (the capacity check of the last bounded pass cleared it)
     BoundedState bs;
     bool assigned = false;
+    // ranked lists (DESIGN.md 3.11): n x ranks row-major, column 0 == idx; ranks == 0 = the set holds none.  The buffer is grow-only
+    // (capacity x ranks), the lists record the policy they were computed under.
+    DevBuf lists;
+    uint32_t ranks = 0, rank_solver = 0, rank_bits = 0;
+    void drop_lists() { ranks = 0; }
 };
 
 namespace {
@@ -1543,7 +1550,7 @@ void rio_cuda_set_destroy(rio_objset *s) {
         std::lock_guard<std::mutex> g(h->mu);
         cudaSetDevice(h->device);
         if (h->aux_stream) cudaStreamSynchronize(h->aux_stream);   // a check of this set may still be in flight
-        s->keys.release(h->stream); s->idx.release(h->stream); s->feats.release(h->stream); s->counters.release(h->stream); s->counters_alt.release(h->stream); s->sel.release(h->stream); s->bs.release(h->stream);
+        s->keys.release(h->stream); s->idx.release(h->stream); s->feats.release(h->stream); s->counters.release(h->stream); s->counters_alt.release(h->stream); s->sel.release(h->stream); s->bs.release(h->stream); s->lists.release(h->stream);
         cudaStreamSynchronize(h->stream);
     }
     delete s;
@@ -1555,7 +1562,7 @@ rio_status rio_cuda_set_load_keys(rio_objset *s, const uint64_t *keys, uint64_t 
     return guarded(h, [&] {
         REQUIRE(n <= s->capacity && (keys || !n), "too many keys for this set");
         CUDA_TRY(cudaMemcpyAsync(s->keys.p, keys, n * 8, cudaMemcpyHostToDevice, h->stream));
-        s->n = n; s->assigned = false;
+        s->n = n; s->assigned = false; s->drop_lists();
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
@@ -1566,7 +1573,7 @@ rio_status rio_cuda_set_synth_keys(rio_objset *s, uint64_t first, uint64_t n, ui
     return guarded(h, [&] {
         REQUIRE(n <= s->capacity, "too many keys for this set");
         launch_synth_keys(h->L(), s->keys.as<uint64_t>(), first, n, seed);
-        s->n = n; s->assigned = false;
+        s->n = n; s->assigned = false; s->drop_lists();
     });
 }
 
@@ -1586,6 +1593,7 @@ rio_status rio_cuda_set_assign(rio_objset *s, uint32_t use_affinity) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
     rio_placement *h = s->h;
     return guarded(h, [&] {
+        s->drop_lists();
         ensure_tab(h);
         set_ensure_counters(s);
         CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
@@ -1602,6 +1610,7 @@ rio_status rio_cuda_set_assign(rio_objset *s, uint32_t use_affinity) {
 static void set_bounded_begin(rio_objset *s, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, bool pipelined) {
     rio_placement *h = s->h;
     REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+    s->drop_lists();
     ensure_tab(h);
     set_ensure_counters(s);
     if (!n_total_objs) n_total_objs = s->n * (uint64_t)h->world;
@@ -1649,6 +1658,7 @@ rio_status rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, u
         REQUIRE(event == RIO_EV_JOIN || event == RIO_EV_LEAVE, "unknown event");
         REQUIRE(idx < h->nodes.size(), "node index out of range");
         REQUIRE(s->assigned, "set has no assignment yet");
+        s->drop_lists();
         ensure_tab(h);
         set_ensure_counters(s);
         zero_scalar(h, S_MOVED);
@@ -1682,6 +1692,7 @@ rio_status rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, co
     return guarded(h, [&] {
         check_change_set(h, idx, prev_weight, k);
         REQUIRE(s->assigned, "set has no assignment yet");
+        s->drop_lists();
         uint64_t moved = 0;
         if (k) {
             ensure_tab(h);
@@ -1708,6 +1719,94 @@ rio_status rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, co
             moved = read_scalar(h, S_MOVED);
         }
         if (out_moved) *out_moved = moved;
+    });
+}
+
+// ---- ranked resident sets (DESIGN.md 3.11) ----------------------------------------------------------------------------------
+namespace {
+
+void require_ranked_set_kernels(uint32_t solver) {
+    const bool have = launch_ranked_primary && launch_assign_hrw_ranked && launch_assign_trie_ranked &&
+                      (solver == RIO_SOLVER_HRW2 ? launch_reassign_trie_ranked != nullptr : launch_rebalance_changes_ranked && launch_scatter_ranked);
+    if (!have) throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked-set kernels (k_ranked_changes.cuh launchers are not linked)"};
+}
+
+}  // namespace
+
+rio_status rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        check_ranked_args(s->n, ranks);
+        require_ranked_set_kernels(h->solver);
+        s->drop_lists();
+        s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
+        set_ensure_counters(s);
+        run_assign_ranked(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
+        launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
+        CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+        launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
+        s->assigned = true;
+        s->ranks = ranks;
+        s->rank_solver = h->solver;
+        s->rank_bits = h->trie_bits;
+    });
+}
+
+rio_status rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(s->ranks, "set holds no ranked lists");
+        REQUIRE(out, "null buffer");
+        REQUIRE(first <= s->n && n <= s->n - first, "range outside the set");
+        if (n) CUDA_TRY(cudaMemcpyAsync(out, s->lists.as<uint32_t>() + first * s->ranks, n * s->ranks * 4, cudaMemcpyDeviceToHost, h->stream));
+        CUDA_TRY(cudaStreamSynchronize(h->stream));
+    });
+}
+
+rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved,
+                                                 uint64_t *out_changed) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        check_change_set(h, idx, prev_weight, k);
+        require_ranked_set_kernels(h->solver);
+        REQUIRE(s->ranks, "set holds no ranked lists");
+        REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
+        const uint32_t R = s->ranks;
+        uint64_t moved = 0, changed = 0;
+        if (k) {
+            ensure_tab(h);
+            set_ensure_counters(s);
+            zero_scalar(h, S_MOVED);
+            zero_scalar(h, S_CHANGED);
+            uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>();
+            if (h->solver == RIO_SOLVER_HRW2) {   // one ranked re-walk of every key, only the changed rows written
+                ensure_rank_tab(h);
+                launch_reassign_trie_ranked(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->rank_tab, R, lists, d_idx, counters, h->tabs.tab.n_total,
+                                            h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+            } else {
+                const ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
+                const ChangeSetDev dcs = upload_change_set(h, cs);
+                zero_scalar(h, S_NSEL);
+                launch_rebalance_changes_ranked(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, counters, s->sel.as<uint32_t>(),
+                                                h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                const uint64_t n_sel = read_scalar(h, S_NSEL);
+                if (n_sel) {   // S1: the selected objects' lists computed afresh over the live set, scattered back
+                    h->s_keys2.ensure(n_sel * 8, h->stream);
+                    h->s_idx.ensure(n_sel * R * 4, h->stream);
+                    launch_gather_keys(h->L(), s->keys.as<uint64_t>(), s->sel.as<uint32_t>(), n_sel, h->s_keys2.as<uint64_t>(), nullptr, nullptr);
+                    launch_assign_hrw_ranked(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, R, h->s_idx.as<uint32_t>());
+                    launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel, R, lists, d_idx, counters, h->tabs.tab.n_total,
+                                          h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                }
+            }
+            moved = read_scalar(h, S_MOVED);
+            changed = read_scalar(h, S_CHANGED);
+        }
+        if (out_moved) *out_moved = moved;
+        if (out_changed) *out_changed = changed;
     });
 }
 

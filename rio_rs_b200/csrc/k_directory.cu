@@ -3,6 +3,7 @@
 // two slots), 128-bit loads on the scans, warp-aggregated counters.
 #include "kernels.cuh"
 #include "k_changes.cuh"
+#include "k_ranked_changes.cuh"
 #include "spec.cuh"
 #include "bounded_tail.cuh"
 
@@ -580,6 +581,143 @@ k_count_changed(const uint32_t *__restrict__ idx, const uint32_t *__restrict__ s
     warp_flush(moved, n_moved);
 }
 
+// ---- ranked resident sets (DESIGN.md 3.11) -------------------------------------------------------------------------------
+// Insert node j (pair hash u, factor r) into the list (gs, gu, gj), best first under the order (E(u)*r, ~u, j) of cand_better: the
+// insertion network of k_assign_hrw_ranked, so ties resolve exactly as there.
+template <int R>
+__device__ __forceinline__ void rank_insert(uint64_t (&gs)[R], uint32_t (&gu)[R], uint32_t (&gj)[R], uint32_t u, uint32_t r, uint32_t j) {
+    uint64_t s = (uint64_t)elog(u) * r;
+    if (!cand_better(s, u, j, gs[R - 1], gu[R - 1], gj[R - 1])) return;
+#pragma unroll
+    for (int y = 0; y < R; y++) {
+        const bool sw = cand_better(s, u, j, gs[y], gu[y], gj[y]);
+        const uint64_t ts = gs[y]; const uint32_t tu = gu[y], tj = gj[y];
+        gs[y] = sw ? s : ts; gu[y] = sw ? u : tu; gj[y] = sw ? j : tj;
+        s = sw ? ts : s; u = sw ? tu : u; j = sw ? tj : j;
+    }
+}
+
+// Flat policy, 8 + 4R B/object: S1 objects (a list member in REPLACE or past the table) are appended to sel; an S2 list becomes the
+// first R of L u CANDIDATES.  When no member of L is a candidate and L is full, its order is unchanged and a candidate enters only by
+// beating L's last member: one pair hash per candidate, behind challenger_wins's clz bracket.  Only then, or when a member gained
+// weight or L is short, is every member and candidate scored and merged.  The trip loop is block-uniform, so the S1 append can ballot.
+template <int R, bool SMEM>
+__global__ void __launch_bounds__(256)
+k_rebalance_changes_ranked(const uint64_t *__restrict__ keys, uint32_t *__restrict__ lists, uint32_t *__restrict__ idx, uint64_t n, NodeTabDev tab,
+                           ChangeSetDev cs_in, uint32_t *__restrict__ counters, uint32_t *__restrict__ sel, unsigned long long *nsel,
+                           unsigned long long *moved, unsigned long long *changed) {
+    const ChangeSetDev cs = stage_changes<SMEM>(cs_in, tab.n_total);
+    const uint4 *by_idx = stage_by_idx<SMEM>(tab);
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    unsigned long long n_moved = 0, n_changed = 0;
+    for (uint64_t b = (uint64_t)blockIdx.x * blockDim.x; b < n; b += stride) {
+        const uint64_t i = b + threadIdx.x;
+        bool s1 = false;
+        if (i < n) {
+            uint32_t l[R];
+#pragma unroll
+            for (int x = 0; x < R; x++) l[x] = lists[i * R + x];
+            const uint64_t key = cs.n_cand ? __ldg(keys + i) : 0;   // no candidate: an S2 list cannot change, the key is not needed
+            bool member_cand = false, full = true;
+#pragma unroll
+            for (int x = 0; x < R; x++) {
+                if (l[x] == kNone) { full = false; continue; }
+                if (l[x] >= tab.n_total) { s1 = true; continue; }
+                const uint8_t f = cs.flag[l[x]];
+                s1 |= (f & kChgReplace) != 0;
+                member_cand |= (f & kChgCandidate) != 0;
+            }
+            if (!s1 && cs.n_cand) {
+                const ObjHash o = obj_hash(key);
+                bool merge = member_cand || !full;
+                if (!merge) {
+                    const uint4 c = by_idx[l[R - 1]];
+                    const uint32_t ul = pair_hash(o, c.x, c.z, c.w);
+                    for (uint32_t q = 0; q < cs.n_cand && !merge; q++) {
+                        const uint32_t j = cs.cand[q];
+                        const uint4 r = by_idx[j];
+                        merge = challenger_wins(pair_hash(o, r.x, r.z, r.w), r.y, j, ul, c.y, l[R - 1]);
+                    }
+                }
+                if (merge) {
+                    uint64_t gs[R];
+                    uint32_t gu[R], gj[R];
+#pragma unroll
+                    for (int x = 0; x < R; x++) { gs[x] = ~0ull; gu[x] = 0; gj[x] = kNone; }
+#pragma unroll
+                    for (int x = 0; x < R; x++) {
+                        if (l[x] == kNone) continue;
+                        const uint4 r = by_idx[l[x]];
+                        rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, l[x]);
+                    }
+                    for (uint32_t q = 0; q < cs.n_cand; q++) {
+                        const uint32_t j = cs.cand[q];
+                        bool in_l = false;
+#pragma unroll
+                        for (int x = 0; x < R; x++) in_l |= l[x] == j;
+                        if (in_l) continue;   // a member that gained weight counts once
+                        const uint4 r = by_idx[j];
+                        rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, j);
+                    }
+                    bool ch = false;
+#pragma unroll
+                    for (int x = 0; x < R; x++) ch |= gj[x] != l[x];
+                    if (ch) {
+#pragma unroll
+                        for (int x = 0; x < R; x++) lists[i * R + x] = gj[x];
+                        n_changed++;
+                        if (gj[0] != l[0]) {
+                            idx[i] = gj[0];
+                            n_moved++;
+                            if (counters) { if (l[0] != kNone) atomicSub(&counters[l[0]], 1u); atomicAdd(&counters[gj[0]], 1u); }
+                        }
+                    }
+                }
+            }
+        }
+        if (__ballot_sync(0xFFFFFFFFu, s1) == 0) continue;
+        const unsigned long long p = warp_reserve(nsel, s1 ? 1u : 0u);
+        if (s1) sel[p] = (uint32_t)i;
+    }
+    warp_flush(moved, n_moved);
+    warp_flush(changed, n_changed);
+}
+
+// S1 objects after the flat ranked kernel re-ranked their gathered keys into fresh (n_sel x R): write back the rows that changed.
+// The stored row still holds the old list, so its column 0 is the old rank 1.
+__global__ void __launch_bounds__(256)
+k_scatter_ranked(const uint32_t *__restrict__ fresh, const uint32_t *__restrict__ sel, uint64_t n_sel, uint32_t ranks, uint32_t *__restrict__ lists,
+                 uint32_t *__restrict__ idx, uint32_t *__restrict__ counters, uint32_t n_total, unsigned long long *moved, unsigned long long *changed) {
+    unsigned long long n_moved = 0, n_changed = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_sel; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t o = __ldg(sel + i);
+        uint32_t *row = lists + o * ranks;
+        const uint32_t *f = fresh + i * ranks;
+        const uint32_t old0 = row[0], new0 = __ldg(f);
+        bool ch = false;
+        for (uint32_t x = 0; x < ranks; x++) {
+            const uint32_t v = __ldg(f + x);
+            if (row[x] != v) { row[x] = v; ch = true; }
+        }
+        n_changed += ch;
+        if (old0 != new0) {
+            idx[o] = new0;
+            n_moved++;
+            if (counters) {
+                if (old0 < n_total) atomicSub(&counters[old0], 1u);
+                if (new0 < n_total) atomicAdd(&counters[new0], 1u);
+            }
+        }
+    }
+    warp_flush(moved, n_moved);
+    warp_flush(changed, n_changed);
+}
+
+__global__ void __launch_bounds__(256)
+k_ranked_primary(const uint32_t *__restrict__ lists, uint64_t n, uint32_t ranks, uint32_t *__restrict__ idx) {
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) idx[i] = __ldg(lists + i * ranks);
+}
+
 // bounded-load rounds: spill selection (DESIGN.md 3.5)
 __global__ void __launch_bounds__(256)
 k_select_spill(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ idx, uint64_t n, const uint32_t *__restrict__ thr,
@@ -826,6 +964,47 @@ void launch_rebalance_changes(const Launch &L, const uint64_t *d_keys, uint32_t 
 void launch_count_changed(const Launch &L, const uint32_t *d_idx, const uint32_t *d_sel, const uint32_t *d_sel_old, uint64_t n_sel, unsigned long long *d_moved) {
     if (!n_sel) return;
     k_count_changed<<<grid_for(n_sel, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_idx, d_sel, d_sel_old, n_sel, d_moved);
+    RIO_COUNT_LAUNCH(L);
+}
+template <int R>
+static void rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
+                                     const ChangeSetDev &cs, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel, unsigned long long *d_moved,
+                                     unsigned long long *d_changed) {
+    const size_t smem = changes_smem(tab, cs);
+    const int grid = grid_for(n, 256, L.sm_count, changes_ctas_per_sm(smem));
+    if (smem) {
+        cudaFuncSetAttribute(k_rebalance_changes_ranked<R, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChangesMaxSmem);
+        k_rebalance_changes_ranked<R, true><<<grid, 256, smem, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed);
+    } else {
+        k_rebalance_changes_ranked<R, false><<<grid, 256, 0, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed);
+    }
+}
+void launch_rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t ranks, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
+                                     const ChangeSetDev &cs, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel, unsigned long long *d_moved,
+                                     unsigned long long *d_changed) {
+    if (!n) return;
+    switch (ranks) {
+        case 1: rebalance_changes_ranked<1>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 2: rebalance_changes_ranked<2>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 3: rebalance_changes_ranked<3>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 4: rebalance_changes_ranked<4>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 5: rebalance_changes_ranked<5>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 6: rebalance_changes_ranked<6>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 7: rebalance_changes_ranked<7>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        case 8: rebalance_changes_ranked<8>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
+        default: return;
+    }
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_scatter_ranked(const Launch &L, const uint32_t *d_fresh, const uint32_t *d_sel, uint64_t n_sel, uint32_t ranks, uint32_t *d_lists, uint32_t *d_idx,
+                           uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {
+    if (!n_sel) return;
+    k_scatter_ranked<<<grid_for(n_sel, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_fresh, d_sel, n_sel, ranks, d_lists, d_idx, d_counters, n_total, d_moved, d_changed);
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_ranked_primary(const Launch &L, const uint32_t *d_lists, uint64_t n, uint32_t ranks, uint32_t *d_idx) {
+    if (!n) return;
+    k_ranked_primary<<<grid_for(n, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_lists, n, ranks, d_idx);
     RIO_COUNT_LAUNCH(L);
 }
 void launch_select_on_node(const Launch &L, const uint32_t *d_idx, uint64_t n, uint32_t node, uint32_t *d_sel, unsigned long long *d_nsel) {

@@ -10,6 +10,7 @@
 //     excluded members and takes each member's "rest" from the bucket weight without the excluded ones.
 // One thread per object; the excluded nodes (index, bucket leaf, weight) stay in registers, R is a template parameter.
 #include "k_ranked.cuh"
+#include "k_ranked_changes.cuh"
 #include "spec.cuh"
 
 namespace rio {
@@ -102,10 +103,19 @@ __device__ __forceinline__ bool contest_left_exact(uint32_t v, unsigned long lon
     return phi < qhi || (phi == qhi && plo <= qlo);
 }
 
-template <int R, bool SMEM>
+// Compare mode (CMP, DESIGN.md 3.11): out_idx holds the stored lists of a resident set.  Each walk is compared with the stored row,
+// only changed rows are written, and the set's primary index and counters follow column 0.  The extra argument comes last, so the
+// plain instantiations keep their parameter layout and code.
+struct RankedCmp {
+    uint32_t *idx, *counters;
+    uint32_t n_total;
+    unsigned long long *moved, *changed;
+};
+
+template <int R, bool SMEM, bool CMP>
 __global__ void __launch_bounds__(kRankThreads)
 k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, TrieRankDev rk, const __grid_constant__ LevelConsts lc,
-                     uint32_t *__restrict__ out_idx) {
+                     uint32_t *__restrict__ out_idx, const RankedCmp cmp) {
     extern __shared__ __align__(16) unsigned char smem_rank[];
     const unsigned char *blob = reinterpret_cast<const unsigned char *>(t.blob);
     const unsigned long long *W = rk.wsum;
@@ -120,6 +130,7 @@ k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, T
     }
     const uint32_t *tab32 = reinterpret_cast<const uint32_t *>(blob);
     const uint32_t bits = t.bits;
+    uint32_t n_moved = 0, n_changed = 0;   // compare mode only (a thread walks far fewer than 2^32 objects)
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         const ObjHash o = obj_hash(__ldg(keys + i));
         uint32_t res[R], xleaf[R], xw[R];   // ranks so far: node index, heap index of its bucket, weight
@@ -191,8 +202,34 @@ k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, T
             }
         }
         uint32_t *dst = out_idx + i * R;
+        if (CMP) {
+            bool changed = false;
 #pragma unroll
-        for (int r = 0; r < R; r++) dst[r] = res[r];
+            for (int r = 0; r < R; r++) changed |= dst[r] != res[r];
+            if (changed) {
+                const uint32_t old0 = dst[0];
+#pragma unroll
+                for (int r = 0; r < R; r++) dst[r] = res[r];
+                n_changed++;
+                if (old0 != res[0]) {
+                    cmp.idx[i] = res[0];
+                    n_moved++;
+                    if (old0 < cmp.n_total) atomicSub(&cmp.counters[old0], 1u);
+                    if (res[0] < cmp.n_total) atomicAdd(&cmp.counters[res[0]], 1u);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int r = 0; r < R; r++) dst[r] = res[r];
+        }
+    }
+    if (CMP) {   // every thread of the block gets here: one atomic per warp and counter
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) { n_moved += __shfl_xor_sync(0xFFFFFFFFu, n_moved, o); n_changed += __shfl_xor_sync(0xFFFFFFFFu, n_changed, o); }
+        if ((threadIdx.x & 31) == 0) {
+            if (n_moved) atomicAdd(cmp.moved, (unsigned long long)n_moved);
+            if (n_changed) atomicAdd(cmp.changed, (unsigned long long)n_changed);
+        }
     }
 }
 
@@ -225,19 +262,23 @@ void hrw_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeT
     }
 }
 
-template <int R>
-void trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t *d_out) {
+template <int R, bool CMP = false>
+void trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t *d_out, const RankedCmp &cmp = {}) {
     static const LevelConsts lc = level_consts();
     const size_t smem = (size_t)t.blob_bytes + rk.bytes;
     if (smem <= kRankSmemBudget) {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, true>, smem, n, attr_set);
-        k_assign_trie_ranked<R, true><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, rk, lc, d_out);
+        const int grid = ranked_grid(L, k_assign_trie_ranked<R, true, CMP>, smem, n, attr_set);
+        k_assign_trie_ranked<R, true, CMP><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
     } else {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, false>, 0, n, attr_set);
-        k_assign_trie_ranked<R, false><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, rk, lc, d_out);
+        const int grid = ranked_grid(L, k_assign_trie_ranked<R, false, CMP>, 0, n, attr_set);
+        k_assign_trie_ranked<R, false, CMP><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
     }
+}
+template <int R>
+void trie_ranked_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t *d_lists, const RankedCmp &cmp) {
+    trie_ranked<R, true>(L, d_keys, n, t, rk, d_lists, cmp);
 }
 
 }  // namespace
@@ -257,6 +298,14 @@ void launch_assign_trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t
                                uint32_t *d_out_idx) {
     if (!n) return;
     RIO_RANK_CASES(trie_ranked, L, d_keys, n, t, rk, d_out_idx)
+    if (L.launch_counter) ++*L.launch_counter;
+}
+
+void launch_reassign_trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t ranks, uint32_t *d_lists,
+                                 uint32_t *d_idx, uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {
+    if (!n) return;
+    const RankedCmp cmp{d_idx, d_counters, n_total, d_moved, d_changed};
+    RIO_RANK_CASES(trie_ranked_cmp, L, d_keys, n, t, rk, d_lists, cmp)
     if (L.launch_counter) ++*L.launch_counter;
 }
 

@@ -548,6 +548,28 @@ class ObjectSet:
         self._ck(self.L.rio_cuda_set_rebalance_changes(self.s, _ptr(idx), _ptr(prev), len(idx), C.byref(m)))
         return m.value
 
+    def assign_ranked(self, ranks):
+        """Each key's first `ranks` nodes under the handle's policy, kept in the set (DESIGN.md 3.11): column 0 becomes the set's
+        assignment (read, counters, commit), the other columns are its standbys.  Calls that assign the set otherwise drop the lists."""
+        self._ck(self.L.rio_cuda_set_assign_ranked(self.s, ranks))
+        self._ranks = int(ranks)
+
+    def read_ranked(self, first=0, n=None):
+        """Rows [first, first + n) of the ranked lists -> (n, ranks) uint32, RIO_NONE past the live set."""
+        if n is None:
+            n = self.size() - first
+        out = np.empty((max(n, 0), getattr(self, "_ranks", 1)), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_set_read_ranked(self.s, first, n, _ptr(out)))
+        return out
+
+    def rebalance_changes_ranked(self, idx, prev_weight):
+        """rebalance_changes for a set holding ranked lists: every list stays equal to the fresh one over the live set.  Returns
+        (moved, changed): objects whose rank 1 changed, and objects whose list changed at any rank."""
+        idx, prev = _change_set(idx, prev_weight)
+        m, c = C.c_uint64(0), C.c_uint64(0)
+        self._ck(self.L.rio_cuda_set_rebalance_changes_ranked(self.s, _ptr(idx), _ptr(prev), len(idx), C.byref(m), C.byref(c)))
+        return m.value, c.value
+
     def counters(self):
         total, _ = self.p.node_count()
         out = np.zeros(max(total, 1), dtype=np.uint32)
