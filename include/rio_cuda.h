@@ -98,6 +98,12 @@ rio_status  rio_cuda_node_address(rio_placement *h, uint32_t idx, char *buf, siz
 rio_status  rio_cuda_node_count(rio_placement *h, uint32_t *out_total, uint32_t *out_live);
 /* membership flag, weight and "address has no ip:port shape" (service.rs:213-222) of an interned node; any out may be NULL */
 rio_status  rio_cuda_node_state(rio_placement *h, uint32_t idx, int32_t *active, uint32_t *weight, int32_t *malformed);
+/* Failure-domain labels (DESIGN.md 3.12): node idx[i] gets label domain[i] (a rack or zone id from the deployment).  RIO_NONE, the
+ * default of every interned node, means "a domain of its own".  Labels stay with the interned index across set_nodes, node_upsert and
+ * node_set_active, count only while the node is live, and change no call other than rio_cuda_assign_ranked_spread_batch.
+ * RIO_ERR_UNKNOWN for an index out of range, a duplicate index, or NULL arrays with k > 0; k == 0 does nothing. */
+rio_status  rio_cuda_node_set_domains(rio_placement *h, const uint32_t *idx, const uint32_t *domain, size_t k);
+rio_status  rio_cuda_node_domain(rio_placement *h, uint32_t idx, uint32_t *out_domain);
 
 /* ---- solver policy of the handle (new; no reference counterpart) ----------------------------------------------------
  * RIO_SOLVER_HRW  = flat weighted rendezvous over all live nodes (DESIGN.md 3.4): M pair hashes per object, minimal movement
@@ -144,6 +150,12 @@ rio_status  rio_cuda_assign_bounded_batch(rio_placement *h, const uint64_t *keys
  * RIO_ERR_UNKNOWN for ranks outside [1, RIO_MAX_RANKS], NULL buffers, or n x ranks overflowing. */
 #define RIO_MAX_RANKS 8u
 rio_status  rio_cuda_assign_ranked_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx);
+/* Ranked placement across failure domains (DESIGN.md 3.12): rank 1 is exactly what assign_batch returns; rank r is the same policy's
+ * placement over the live set minus every node whose domain is the domain of one of ranks 1..r-1.  The ranks lie in distinct
+ * domains, rank 2 is where the object goes when rank 1's whole domain leaves, and the entries past the number of distinct live
+ * domains are RIO_NONE.  With no labels set the result equals rio_cuda_assign_ranked_batch.  Output and argument errors as for
+ * rio_cuda_assign_ranked_batch; RIO_ERR_UPSTREAM when the library was built without the spread kernels. */
+rio_status  rio_cuda_assign_ranked_spread_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx);
 /* Ranked placement under the affinity cost (DESIGN.md 3.9): each object's `ranks` lowest-cost live nodes, cost = -dot(F_obj, F_node),
  * in increasing (cost, node index) order.  rank 1 is exactly what assign_batch with the same obj_feats returns; rank r is the
  * affinity placement over the live set minus ranks 1..r-1, so rank 2 is where a LEAVE of rank 1 sends the object.  obj_feats is
@@ -271,6 +283,7 @@ rio_status  rio_cuda_memcpy_d2h(rio_placement *h, void *host, const void *dev, s
 rio_status  rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, const float *d_obj_feats,
                                       size_t n, uint32_t *d_out_idx);
 rio_status  rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx);
+rio_status  rio_cuda_assign_ranked_spread_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_lookup_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t *d_out_idx);
 rio_status  rio_cuda_upsert_batch_dev(rio_placement *h, const uint64_t *d_keys, const uint32_t *d_idx, size_t n);

@@ -51,6 +51,8 @@ SIGNATURES = {
     "rio_cuda_node_address": (C.c_int32, [H, C.c_uint32, C.c_char_p, sz, C.POINTER(sz)]),
     "rio_cuda_node_count": (C.c_int32, [H, u32p, u32p]),
     "rio_cuda_node_state": (C.c_int32, [H, C.c_uint32, C.POINTER(C.c_int32), u32p, C.POINTER(C.c_int32)]),
+    "rio_cuda_node_set_domains": (C.c_int32, [H, vp, vp, sz]),
+    "rio_cuda_node_domain": (C.c_int32, [H, C.c_uint32, u32p]),
     "rio_cuda_set_solver": (C.c_int32, [H, C.c_uint32, C.c_uint32]),
     "rio_cuda_get_solver": (C.c_int32, [H, u32p, u32p]),
     "rio_cuda_lookup_batch": (C.c_int32, [H, vp, sz, vp]),
@@ -62,6 +64,8 @@ SIGNATURES = {
     "rio_cuda_assign_bounded_batch": (C.c_int32, [H, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p]),
     "rio_cuda_assign_ranked_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
+    "rio_cuda_assign_ranked_spread_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
+    "rio_cuda_assign_ranked_spread_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_affinity_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_affinity_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_check_address_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp, u64p]),

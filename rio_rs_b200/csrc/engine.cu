@@ -11,6 +11,7 @@
 #include "k_affinity_ranked.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
+#include "k_spread.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -110,6 +111,7 @@ struct NodeInfo {
     std::string addr;
     uint64_t seed = 0, seed2 = 0;
     uint32_t weight = 0;
+    uint32_t domain = RIO_NONE;   // failure-domain label (DESIGN.md 3.12); RIO_NONE = a domain of its own
     bool active = false;
     bool malformed = false;
     std::vector<float> feat;
@@ -189,6 +191,13 @@ struct rio_placement {
     std::vector<unsigned char> rank_stage;
     TrieRankDev rank_tab{};
     uint64_t rank_version = ~0ull;            // tab_version the side table belongs to
+    // side table of the spread walks (DESIGN.md 3.12): built on the first spread call after a table or label change.  Labels never
+    // touch tab_version: no other call depends on them.
+    uint64_t label_version = 0;
+    DevBuf spread_dev;
+    std::vector<unsigned char> spread_stage;
+    SpreadTabDev spread_tab{};
+    uint64_t spread_version[2] = {~0ull, ~0ull};   // (tab_version, label_version) the side table belongs to
     unsigned long long *d_scalars = nullptr;   // S_COUNT u64 + error u32
     unsigned long long *h_scalars = nullptr;   // pinned mirror
 
@@ -549,6 +558,80 @@ void run_assign_ranked(rio_placement *h, const uint64_t *d_keys, uint64_t n, uin
     } else {
         launch_assign_hrw_ranked(h->L(), d_keys, n, h->tabs.tab, ranks, d_out_idx);
     }
+}
+
+// The spread walks need the ranked side table plus the live members grouped by domain: dense domain ids (one per label shared by
+// live nodes, one per live node labelled RIO_NONE), the members sorted by (domain, bucket, index) with a running weight, and for the
+// flat kernel the domain of every record in the class-sorted order build_tab gives the table, (inverse weight, node index).
+void ensure_spread_tab(rio_placement *h) {
+    if (h->spread_version[0] == h->tab_version && h->spread_version[1] == h->label_version) return;
+    const uint32_t n_total = (uint32_t)h->nodes.size();
+    std::vector<TrieMember> members;
+    std::vector<uint32_t> live, ndom(n_total, kNone);
+    std::unordered_map<uint32_t, uint32_t> dense;
+    uint32_t n_dom = 0;
+    for (uint32_t j = 0; j < n_total; j++) {
+        const NodeInfo &ni = h->nodes[j];
+        if (!ni.live()) continue;
+        members.push_back(TrieMember{ni.seed, j, ni.weight});
+        live.push_back(j);
+        if (ni.domain == RIO_NONE) ndom[j] = n_dom++;
+        else ndom[j] = dense.emplace(ni.domain, n_dom).second ? n_dom++ : dense[ni.domain];
+    }
+    const TrieBlob blob = build_trie_blob(members, h->trie_bits);
+    const uint32_t bits = blob.bits, nb = 1u << bits, n_live = (uint32_t)live.size();
+    std::vector<uint32_t> bucket(n_total, 0);
+    for (uint32_t j : live) bucket[j] = bits ? (uint32_t)(mix64(h->nodes[j].seed ^ kSaltPos) >> (64 - bits)) : 0u;
+    std::vector<uint32_t> by_dom(live), by_class(live);
+    std::sort(by_dom.begin(), by_dom.end(), [&](uint32_t a, uint32_t b) {
+        return ndom[a] != ndom[b] ? ndom[a] < ndom[b] : bucket[a] != bucket[b] ? bucket[a] < bucket[b] : a < b;
+    });
+    std::stable_sort(by_class.begin(), by_class.end(), [&](uint32_t a, uint32_t b) { return inv_weight(h->nodes[a].weight) < inv_weight(h->nodes[b].weight); });
+    auto al = [](size_t v) { return (v + 15) / 16 * 16; };
+    SpreadTabDev sp{};
+    sp.o_node = nb * 16u;
+    sp.o_ndom = (uint32_t)(sp.o_node + al((size_t)n_total * 8));
+    sp.o_pre = (uint32_t)(sp.o_ndom + al((size_t)n_total * 4));
+    sp.o_mb = (uint32_t)(sp.o_pre + al(((size_t)n_live + 1) * 8));
+    sp.o_dstart = (uint32_t)(sp.o_mb + al((size_t)n_live * 4));
+    sp.trie_bytes = (uint32_t)(sp.o_dstart + al(((size_t)n_dom + 1) * 4));
+    sp.n_members = n_live;
+    sp.n_domains = n_dom;
+    const size_t total = sp.trie_bytes + al((size_t)n_live * 4);
+    h->spread_stage.assign(total, 0);
+    unsigned char *st8 = h->spread_stage.data();
+    memcpy(st8, blob.wsum.data(), (size_t)nb * 16);
+    uint2 *node = reinterpret_cast<uint2 *>(st8 + sp.o_node);
+    for (uint32_t j : live) node[j] = make_uint2(bucket[j], h->nodes[j].weight);
+    memcpy(st8 + sp.o_ndom, ndom.data(), (size_t)n_total * 4);
+    uint64_t *pre = reinterpret_cast<uint64_t *>(st8 + sp.o_pre);
+    uint32_t *mb = reinterpret_cast<uint32_t *>(st8 + sp.o_mb), *dstart = reinterpret_cast<uint32_t *>(st8 + sp.o_dstart);
+    uint32_t *pos_dom = reinterpret_cast<uint32_t *>(st8 + sp.trie_bytes);
+    for (uint32_t q = 0; q < n_live; q++) {
+        const uint32_t j = by_dom[q];
+        pre[q + 1] = pre[q] + h->nodes[j].weight;
+        mb[q] = bucket[j];
+        dstart[ndom[j] + 1] = q + 1;
+        pos_dom[q] = ndom[by_class[q]];
+    }
+    cudaStream_t st = h->stream;
+    h->spread_dev.ensure(total, st);
+    CUDA_TRY(cudaMemcpyAsync(h->spread_dev.p, st8, total, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    sp.base = h->spread_dev.as<unsigned char>();
+    h->spread_tab = sp;
+    h->spread_version[0] = h->tab_version;
+    h->spread_version[1] = h->label_version;
+}
+
+// each object's first `ranks` nodes in distinct failure domains under the handle's policy (DESIGN.md 3.12)
+void run_assign_spread(rio_placement *h, const uint64_t *d_keys, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!launch_assign_hrw_spread || !launch_assign_trie_spread)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no spread kernels (k_spread.cu is not linked)"};
+    ensure_tab(h);
+    ensure_spread_tab(h);
+    if (h->solver == RIO_SOLVER_HRW2) launch_assign_trie_spread(h->L(), d_keys, n, h->tabs.trie, h->spread_tab, ranks, d_out_idx);
+    else launch_assign_hrw_spread(h->L(), d_keys, n, h->tabs.tab, h->spread_tab, ranks, d_out_idx);
 }
 
 // affinity dispatch: tensor-core (wgmma) kernel for K == 16 (unless RIO_AFFINITY_VARIANT=ffma or the node set does not fit), else CUDA cores
@@ -936,7 +1019,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev, &h->spread_dev};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -1054,6 +1137,31 @@ rio_status rio_cuda_node_intern(rio_placement *h, const char *address, uint32_t 
     return guarded(h, [&] {
         REQUIRE(address && out_idx, "null argument");
         *out_idx = intern_node(h, address);
+    });
+}
+
+rio_status rio_cuda_node_set_domains(rio_placement *h, const uint32_t *idx, const uint32_t *domain, size_t k) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        if (!k) return;
+        REQUIRE(idx && domain, "null domain arrays");
+        std::vector<uint8_t> seen(h->nodes.size(), 0);
+        for (size_t i = 0; i < k; i++) {
+            REQUIRE(idx[i] < h->nodes.size(), "node index out of range");
+            REQUIRE(!seen[idx[i]], "duplicate node index");
+            seen[idx[i]] = 1;
+        }
+        for (size_t i = 0; i < k; i++) h->nodes[idx[i]].domain = domain[i];
+        h->label_version++;
+    });
+}
+
+rio_status rio_cuda_node_domain(rio_placement *h, uint32_t idx, uint32_t *out_domain) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        REQUIRE(out_domain, "null argument");
+        REQUIRE(idx < h->nodes.size(), "node index out of range");
+        *out_domain = h->nodes[idx].domain;
     });
 }
 
@@ -1266,6 +1374,32 @@ rio_status rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_
         if (!n) return;
         REQUIRE(d_keys && d_out_idx, "null buffer");
         run_assign_ranked(h, d_keys, n, ranks, d_out_idx);
+    });
+}
+
+rio_status rio_cuda_assign_ranked_spread_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(keys && out_idx, "null buffer");
+        cudaStream_t st = h->stream;
+        h->s_keys.ensure(n * 8, st);
+        h->s_idx.ensure(n * ranks * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
+        run_assign_spread(h, h->s_keys.as<uint64_t>(), n, ranks, h->s_idx.as<uint32_t>());
+        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+    });
+}
+
+rio_status rio_cuda_assign_ranked_spread_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(d_keys && d_out_idx, "null buffer");
+        run_assign_spread(h, d_keys, n, ranks, d_out_idx);
     });
 }
 

@@ -9,6 +9,7 @@
 //     with the exact compare LEFT <=> (v+1)(wl'+wr') <= 2^31 wl' (a 64x64->128 product, no division).  A bucket's chain skips
 //     excluded members and takes each member's "rest" from the bucket weight without the excluded ones.
 // One thread per object; the excluded nodes (index, bucket leaf, weight) stay in registers, R is a template parameter.
+#include "k_rank_common.cuh"
 #include "k_ranked.cuh"
 #include "k_ranked_changes.cuh"
 #include "spec.cuh"
@@ -17,28 +18,7 @@ namespace rio {
 
 namespace {
 
-constexpr int kRankThreads = 256;
-constexpr uint32_t kRankLevels = 16;
 constexpr uint32_t kRankSmemBudget = 200u * 1024u;
-
-// per-level contest constants (pseudo-node seeds c_l, DESIGN.md 3.8), passed by value: spec constants, the same for every handle
-struct LevelConsts { uint32_t s0[kRankLevels], m2[kRankLevels], h2[kRankLevels]; };
-
-LevelConsts level_consts() {
-    LevelConsts c{};
-    for (uint32_t l = 0; l < kRankLevels; l++) {
-        const ContestRec r = contest_rec(level_seed(l));
-        c.s0[l] = r.s0; c.m2[l] = r.m2; c.h2[l] = r.h2;
-    }
-    return c;
-}
-
-// 16-byte cooperative copy into shared memory (bytes is a multiple of 16)
-__device__ __forceinline__ void stage16(unsigned char *dst, const void *src, uint32_t bytes) {
-    const uint4 *s = reinterpret_cast<const uint4 *>(src);
-    uint4 *d = reinterpret_cast<uint4 *>(dst);
-    for (uint32_t i = threadIdx.x; i < bytes / 16; i += blockDim.x) d[i] = __ldg(s + i);
-}
 
 // ---- flat weighted rendezvous ------------------------------------------------------------------------------------------
 template <int R, bool SMEM>
@@ -95,14 +75,6 @@ k_assign_hrw_ranked(const uint64_t *__restrict__ keys, uint64_t n, NodeTabDev ta
 }
 
 // ---- HRW2 ----------------------------------------------------------------------------------------------------------------
-// v < floor(2^31 wl / (wl + wr))  <=>  (v + 1)(wl + wr) <= 2^31 wl, exactly; wl = 0 never takes LEFT, wr = 0 always does
-__device__ __forceinline__ bool contest_left_exact(uint32_t v, unsigned long long wl, unsigned long long wr) {
-    const unsigned long long a = (unsigned long long)v + 1ull, s = wl + wr;
-    const unsigned long long plo = a * s, phi = __umul64hi(a, s);
-    const unsigned long long qlo = wl << 31, qhi = wl >> 33;
-    return phi < qhi || (phi == qhi && plo <= qlo);
-}
-
 // Compare mode (CMP, DESIGN.md 3.11): out_idx holds the stored lists of a resident set.  Each walk is compared with the stored row,
 // only changed rows are written, and the set's primary index and counters follow column 0.  The extra argument comes last, so the
 // plain instantiations keep their parameter layout and code.
@@ -233,31 +205,16 @@ k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, T
     }
 }
 
-// attr_set: one flag per device for THIS kernel instantiation (the attribute call costs ~1 us of host time per launch otherwise)
-template <class K>
-int ranked_grid(const Launch &L, K kern, size_t smem, uint64_t n, bool (&attr_set)[64]) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRankSmemBudget);
-        if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
-    int per_sm = 0;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kRankThreads, smem);
-    const uint64_t blocks = (n + kRankThreads - 1) / kRankThreads, cap = (uint64_t)L.sm_count * (uint64_t)(per_sm > 0 ? per_sm : 1);
-    return (int)(blocks < cap ? blocks : cap);
-}
-
 template <int R>
 void hrw_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeTabDev &tab, uint32_t *d_out) {
     const size_t smem = (size_t)tab.n_live * 16;
     if (smem <= 96u * 1024u) {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, true>, smem, n, attr_set);
+        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, true>, smem, kRankSmemBudget, n, attr_set);
         k_assign_hrw_ranked<R, true><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, tab, d_out);
     } else {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, false>, 0, n, attr_set);
+        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, false>, 0, kRankSmemBudget, n, attr_set);
         k_assign_hrw_ranked<R, false><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, tab, d_out);
     }
 }
@@ -268,11 +225,11 @@ void trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const Trie
     const size_t smem = (size_t)t.blob_bytes + rk.bytes;
     if (smem <= kRankSmemBudget) {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, true, CMP>, smem, n, attr_set);
+        const int grid = ranked_grid(L, k_assign_trie_ranked<R, true, CMP>, smem, kRankSmemBudget, n, attr_set);
         k_assign_trie_ranked<R, true, CMP><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
     } else {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, false, CMP>, 0, n, attr_set);
+        const int grid = ranked_grid(L, k_assign_trie_ranked<R, false, CMP>, 0, kRankSmemBudget, n, attr_set);
         k_assign_trie_ranked<R, false, CMP><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
     }
 }
@@ -282,11 +239,6 @@ void trie_ranked_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const 
 }
 
 }  // namespace
-
-#define RIO_RANK_CASES(F, ...) \
-    switch (ranks) { case 1: F<1>(__VA_ARGS__); break; case 2: F<2>(__VA_ARGS__); break; case 3: F<3>(__VA_ARGS__); break; \
-                     case 4: F<4>(__VA_ARGS__); break; case 5: F<5>(__VA_ARGS__); break; case 6: F<6>(__VA_ARGS__); break; \
-                     case 7: F<7>(__VA_ARGS__); break; case 8: F<8>(__VA_ARGS__); break; default: return; }
 
 void launch_assign_hrw_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeTabDev &tab, uint32_t ranks, uint32_t *d_out_idx) {
     if (!n) return;
@@ -308,7 +260,5 @@ void launch_reassign_trie_ranked(const Launch &L, const uint64_t *d_keys, uint64
     RIO_RANK_CASES(trie_ranked_cmp, L, d_keys, n, t, rk, d_lists, cmp)
     if (L.launch_counter) ++*L.launch_counter;
 }
-
-#undef RIO_RANK_CASES
 
 }  // namespace rio

@@ -95,6 +95,12 @@ class GpuObjectPlacement {
         return out;
     }
     void node_set_active(uint32_t idx, bool active) const { check(rio_cuda_node_set_active(e_->h, idx, active)); }
+    // failure-domain labels (DESIGN.md 3.12): a rack or zone id per node, RIO_NONE = a domain of its own
+    void set_node_domains(const std::vector<uint32_t> &idx, const std::vector<uint32_t> &domain) const {
+        if (idx.size() != domain.size()) throw ObjectPlacementError(ObjectPlacementError::Unknown, "idx and domain differ in length");
+        check(rio_cuda_node_set_domains(e_->h, idx.data(), domain.data(), idx.size()));
+    }
+    uint32_t node_domain(uint32_t idx) const { uint32_t d = RIO_NONE; check(rio_cuda_node_domain(e_->h, idx, &d)); return d; }
     std::string node_address(uint32_t idx) const {
         size_t len = 0;
         check(rio_cuda_node_address(e_->h, idx, nullptr, 0, &len));      // the length first, then the bytes
@@ -119,6 +125,12 @@ class GpuObjectPlacement {
     std::vector<uint32_t> assign_ranked(const std::vector<uint64_t> &keys, uint32_t ranks) const {
         std::vector<uint32_t> out(keys.size() * ranks);
         check(rio_cuda_assign_ranked_batch(e_->h, keys.data(), keys.size(), ranks, out.data()));
+        return out;
+    }
+    // each object's first `ranks` nodes in distinct failure domains (DESIGN.md 3.12), row-major as for assign_ranked
+    std::vector<uint32_t> assign_ranked_spread(const std::vector<uint64_t> &keys, uint32_t ranks) const {
+        std::vector<uint32_t> out(keys.size() * ranks);
+        check(rio_cuda_assign_ranked_spread_batch(e_->h, keys.data(), keys.size(), ranks, out.data()));
         return out;
     }
     // each object's `ranks` lowest-cost live nodes under the affinity cost (DESIGN.md 3.9); obj_feats is n x K row-major (K of

@@ -286,6 +286,27 @@ class GpuObjectPlacement:
         self._ck(self.L.rio_cuda_assign_ranked_batch(self.h, _ptr(keys), len(keys), ranks, _ptr(out)))
         return out
 
+    def set_node_domains(self, idx, domain):
+        """Failure-domain labels (DESIGN.md 3.12): node idx[i] gets label domain[i] (a rack or zone id); N.NONE = a domain of its own."""
+        idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        dom = np.ascontiguousarray(domain, dtype=np.uint32)
+        if idx.shape != dom.shape or idx.ndim != 1:
+            raise Unknown("idx and domain must be 1-D arrays of one length")
+        self._ck(self.L.rio_cuda_node_set_domains(self.h, _ptr(idx), _ptr(dom), len(idx)))
+
+    def node_domain(self, idx):
+        d = C.c_uint32(0)
+        self._ck(self.L.rio_cuda_node_domain(self.h, idx, C.byref(d)))
+        return d.value
+
+    def assign_ranked_spread(self, keys, ranks):
+        """Each object's first `ranks` nodes in distinct failure domains (DESIGN.md 3.12) -> (n, ranks) uint32: column 0 is
+        assign_batch, column 1 where the object goes when column 0's whole domain leaves; RIO_NONE past the live domain count."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        out = np.empty((len(keys), ranks), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_assign_ranked_spread_batch(self.h, _ptr(keys), len(keys), ranks, _ptr(out)))
+        return out
+
     def assign_ranked_affinity(self, obj_feats, ranks):
         """Each object's `ranks` lowest-cost live nodes under the affinity cost (DESIGN.md 3.9) -> (n, ranks) uint32: column 0 is
         assign_batch(obj_feats=...), column 1 where a LEAVE of column 0 sends the object; RIO_NONE past the live set."""

@@ -147,6 +147,27 @@ impl GpuObjectPlacement {
         check(self.h(), unsafe { sys::rio_cuda_assign_ranked_batch(self.h(), keys.as_ptr(), keys.len(), ranks, out.as_mut_ptr()) })?;
         Ok(out)
     }
+    /// Each object's first `ranks` nodes in distinct failure domains (DESIGN.md 3.12), row-major as for `assign_ranked`.  Rank 2
+    /// is where the object goes when rank 1's whole domain leaves; entries past the number of live domains are `RIO_NONE`.
+    pub fn assign_ranked_spread(&self, keys: &[u64], ranks: u32) -> Result<Vec<u32>, ObjectPlacementError> {
+        let len = keys.len().checked_mul(ranks as usize).ok_or_else(|| ObjectPlacementError::Unknown("n x ranks overflows".into()))?;
+        let mut out = vec![sys::RIO_NONE; len];
+        check(self.h(), unsafe { sys::rio_cuda_assign_ranked_spread_batch(self.h(), keys.as_ptr(), keys.len(), ranks, out.as_mut_ptr()) })?;
+        Ok(out)
+    }
+    /// Failure-domain labels (DESIGN.md 3.12): node `idx[i]` gets `domain[i]`, a rack or zone id; `RIO_NONE` is a domain of its own.
+    pub fn set_node_domains(&self, idx: &[u32], domain: &[u32]) -> Result<(), ObjectPlacementError> {
+        if idx.len() != domain.len() {
+            return Err(ObjectPlacementError::Unknown("idx and domain differ in length".into()));
+        }
+        check(self.h(), unsafe { sys::rio_cuda_node_set_domains(self.h(), idx.as_ptr(), domain.as_ptr(), idx.len()) })
+    }
+    /// The failure-domain label of an interned node (`RIO_NONE` if none was set).
+    pub fn node_domain(&self, idx: u32) -> Result<u32, ObjectPlacementError> {
+        let mut d = sys::RIO_NONE;
+        check(self.h(), unsafe { sys::rio_cuda_node_domain(self.h(), idx, &mut d) })?;
+        Ok(d)
+    }
     /// Each object's `ranks` lowest-cost live nodes under the affinity cost (DESIGN.md 3.9).  `obj_feats` is `n x K` row-major
     /// (K of set_nodes); the result is row-major as for `assign_ranked`, and rank 1 is `assign_batch` with the same features.
     pub fn assign_ranked_affinity(&self, obj_feats: &[f32], n: usize, ranks: u32) -> Result<Vec<u32>, ObjectPlacementError> {

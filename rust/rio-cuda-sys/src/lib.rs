@@ -63,6 +63,8 @@ extern "C" {
     pub fn rio_cuda_assign_bounded_batch(h: *mut rio_placement, keys: *const u64, n: usize, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_check_address_batch(h: *mut rio_placement, addr_idx: *const u32, n: usize, self_idx: u32, out_verdict: *mut u8, out_cleaned: *mut u64) -> rio_status;
     pub fn rio_cuda_node_state(h: *mut rio_placement, idx: u32, active: *mut i32, weight: *mut u32, malformed: *mut i32) -> rio_status;
+    pub fn rio_cuda_node_set_domains(h: *mut rio_placement, idx: *const u32, domain: *const u32, k: size_t) -> rio_status;
+    pub fn rio_cuda_node_domain(h: *mut rio_placement, idx: u32, out_domain: *mut u32) -> rio_status;
     pub fn rio_cuda_set_solver(h: *mut rio_placement, solver: u32, trie_bits: u32) -> rio_status;
     pub fn rio_cuda_get_solver(h: *mut rio_placement, solver: *mut u32, trie_bits: *mut u32) -> rio_status;
 
@@ -75,6 +77,7 @@ extern "C" {
 
     pub fn rio_cuda_assign_batch(h: *mut rio_placement, keys: *const u64, obj_feats: *const f32, n: size_t, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_batch(h: *mut rio_placement, keys: *const u64, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_spread_batch(h: *mut rio_placement, keys: *const u64, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_affinity_batch(h: *mut rio_placement, obj_feats: *const f32, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_place_batch(h: *mut rio_placement, keys: *const u64, n: size_t, policy: u32, self_idx: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_rebalance(h: *mut rio_placement, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
@@ -115,6 +118,7 @@ extern "C" {
     pub fn rio_cuda_memcpy_d2h(h: *mut rio_placement, host: *mut c_void, dev: *const c_void, bytes: size_t) -> rio_status;
     pub fn rio_cuda_assign_batch_dev(h: *mut rio_placement, d_keys: *const u64, d_obj_feats: *const f32, n: size_t, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_spread_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_affinity_batch_dev(h: *mut rio_placement, d_obj_feats: *const f32, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_lookup_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_upsert_batch_dev(h: *mut rio_placement, d_keys: *const u64, d_idx: *const u32, n: size_t) -> rio_status;
