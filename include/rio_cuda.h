@@ -252,6 +252,15 @@ rio_status  rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks);
 rio_status  rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out);
 rio_status  rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t *out_moved,
                                                   uint64_t *out_changed);
+/* Failure-domain resident sets (DESIGN.md 3.13).  rio_cuda_set_assign_ranked_spread works as rio_cuda_set_assign_ranked, with each
+ * key's failure-domain list (as rio_cuda_assign_ranked_spread_batch computes it) in place of its ranked list, and also records the
+ * label of every interned node.  rio_cuda_set_read_ranked reads these lists unchanged.  On such a set
+ * rio_cuda_set_rebalance_changes_ranked leaves every list equal to the fresh failure-domain list over the current live set and the
+ * CURRENT labels: relabels made since the labels were recorded belong to the change set, so k = 0 with a relabel applies it, and
+ * k = 0 without one does nothing.  A successful call records the labels again.  Errors as for the ranked sets; RIO_ERR_UPSTREAM
+ * when the library was built without the spread-set kernels.  The calls that drop ranked lists drop these too, and
+ * rio_cuda_set_assign_ranked makes the set a plain ranked set again (plain ranked sets ignore labels). */
+rio_status  rio_cuda_set_assign_ranked_spread(rio_objset *s, uint32_t ranks);
 /* Global (all ranks) per-node counters of the set's current assignment. */
 rio_status  rio_cuda_set_counters(rio_objset *s, uint32_t *out, uint32_t cap);
 rio_status  rio_cuda_set_read(rio_objset *s, uint64_t first, uint64_t n, uint64_t *out_keys, uint32_t *out_idx);

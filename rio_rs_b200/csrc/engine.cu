@@ -12,6 +12,7 @@
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
+#include "k_spread_changes.cuh"
 #include "spec.cuh"
 #include "trie_table.hpp"
 
@@ -232,7 +233,12 @@ struct rio_objset {
     // (capacity x ranks), the lists record the policy they were computed under.
     DevBuf lists;
     uint32_t ranks = 0, rank_solver = 0, rank_bits = 0;
-    void drop_lists() { ranks = 0; }
+    // spread lists (DESIGN.md 3.13): the lists are failure-domain lists, computed under the labels of label_snap (one per node interned
+    // then; a node interned later had RIO_NONE), which were the handle's labels at label_version label_snap_version
+    bool spread = false;
+    std::vector<uint32_t> label_snap;
+    uint64_t label_snap_version = 0;
+    void drop_lists() { ranks = 0; spread = false; }
 };
 
 namespace {
@@ -1609,6 +1615,20 @@ ChangeSetHost build_change_set(const rio_placement *h, const uint32_t *idx, cons
     return cs;
 }
 
+// Spread lists (DESIGN.md 3.13): a relabelled live node is REPLACE | CANDIDATE.  Lists holding it are recomputed; every other list
+// considers it under its new label.
+void add_relabels(ChangeSetHost &cs, const std::vector<uint32_t> &relabelled) {
+    for (uint32_t j : relabelled) {
+        if (!(cs.bytes[j] & kChgCandidate)) {
+            const size_t o = cs.bytes.size();
+            cs.bytes.resize(o + 4);
+            memcpy(cs.bytes.data() + o, &j, 4);
+            cs.n_cand++;
+        }
+        cs.bytes[j] = kChgReplace | kChgCandidate;
+    }
+}
+
 ChangeSetDev upload_change_set(rio_placement *h, const ChangeSetHost &cs) {
     h->s_misc.ensure(cs.bytes.size(), h->stream);
     CUDA_TRY(cudaMemcpyAsync(h->s_misc.p, cs.bytes.data(), cs.bytes.size(), cudaMemcpyHostToDevice, h->stream));
@@ -1865,26 +1885,65 @@ void require_ranked_set_kernels(uint32_t solver) {
     if (!have) throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked-set kernels (k_ranked_changes.cuh launchers are not linked)"};
 }
 
+void require_spread_set_kernels(uint32_t solver) {
+    const bool have = launch_ranked_primary && launch_assign_hrw_spread && launch_assign_trie_spread &&
+                      (solver == RIO_SOLVER_HRW2 ? launch_reassign_trie_spread != nullptr : launch_rebalance_changes_spread && launch_scatter_ranked);
+    if (!have) throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no spread-set kernels (k_spread_changes.cuh launchers are not linked)"};
+}
+
+// the handle's labels become the set's snapshot (DESIGN.md 3.13)
+void snapshot_labels(rio_objset *s) {
+    const rio_placement *h = s->h;
+    s->label_snap.resize(h->nodes.size());
+    for (size_t j = 0; j < h->nodes.size(); j++) s->label_snap[j] = h->nodes[j].domain;
+    s->label_snap_version = h->label_version;
+}
+
+// live nodes whose label differs from the set's snapshot; a node interned after the snapshot had RIO_NONE there
+std::vector<uint32_t> relabelled_live(const rio_objset *s) {
+    const rio_placement *h = s->h;
+    std::vector<uint32_t> out;
+    if (s->label_snap_version == h->label_version) return out;
+    for (uint32_t j = 0; j < (uint32_t)h->nodes.size(); j++) {
+        const uint32_t was = j < s->label_snap.size() ? s->label_snap[j] : RIO_NONE;
+        if (h->nodes[j].domain != was && h->nodes[j].live()) out.push_back(j);
+    }
+    return out;
+}
+
+// set_assign_ranked (3.11) and set_assign_ranked_spread (3.13): fresh lists, column 0 into idx, the counters rebuilt from it, and the
+// policy (and for spread lists the labels) they were computed under recorded
+void set_assign_lists(rio_objset *s, uint32_t ranks, bool spread) {
+    rio_placement *h = s->h;
+    check_ranked_args(s->n, ranks);
+    if (spread) require_spread_set_kernels(h->solver);
+    else require_ranked_set_kernels(h->solver);
+    s->drop_lists();
+    s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
+    set_ensure_counters(s);
+    if (spread) run_assign_spread(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
+    else run_assign_ranked(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
+    launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
+    CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+    launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
+    s->assigned = true;
+    s->ranks = ranks;
+    s->rank_solver = h->solver;
+    s->rank_bits = h->trie_bits;
+    s->spread = spread;
+    if (spread) snapshot_labels(s);
+}
+
 }  // namespace
 
 rio_status rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
-    rio_placement *h = s->h;
-    return guarded(h, [&] {
-        check_ranked_args(s->n, ranks);
-        require_ranked_set_kernels(h->solver);
-        s->drop_lists();
-        s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
-        set_ensure_counters(s);
-        run_assign_ranked(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
-        launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
-        CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
-        launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
-        s->assigned = true;
-        s->ranks = ranks;
-        s->rank_solver = h->solver;
-        s->rank_bits = h->trie_bits;
-    });
+    return guarded(s->h, [&] { set_assign_lists(s, ranks, false); });
+}
+
+rio_status rio_cuda_set_assign_ranked_spread(rio_objset *s, uint32_t ranks) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    return guarded(s->h, [&] { set_assign_lists(s, ranks, true); });
 }
 
 rio_status rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out) {
@@ -1905,33 +1964,49 @@ rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *
     rio_placement *h = s->h;
     return guarded(h, [&] {
         check_change_set(h, idx, prev_weight, k);
-        require_ranked_set_kernels(h->solver);
+        const bool spread = s->spread;   // the kind of lists the set holds (false when it holds none)
+        if (spread) require_spread_set_kernels(h->solver);
+        else require_ranked_set_kernels(h->solver);
         REQUIRE(s->ranks, "set holds no ranked lists");
         REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
         const uint32_t R = s->ranks;
         uint64_t moved = 0, changed = 0;
-        if (k) {
+        // spread lists: the relabels since the snapshot belong to the change set (DESIGN.md 3.13)
+        const std::vector<uint32_t> relabelled = spread ? relabelled_live(s) : std::vector<uint32_t>{};
+        if (k || !relabelled.empty()) {
             ensure_tab(h);
+            if (spread) ensure_spread_tab(h);
             set_ensure_counters(s);
             zero_scalar(h, S_MOVED);
             zero_scalar(h, S_CHANGED);
             uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>();
             if (h->solver == RIO_SOLVER_HRW2) {   // one ranked re-walk of every key, only the changed rows written
-                ensure_rank_tab(h);
-                launch_reassign_trie_ranked(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->rank_tab, R, lists, d_idx, counters, h->tabs.tab.n_total,
-                                            h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                if (spread) {
+                    launch_reassign_trie_spread(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->spread_tab, R, lists, d_idx, counters,
+                                                h->tabs.tab.n_total, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                } else {
+                    ensure_rank_tab(h);
+                    launch_reassign_trie_ranked(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->rank_tab, R, lists, d_idx, counters, h->tabs.tab.n_total,
+                                                h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                }
             } else {
-                const ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
+                ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
+                add_relabels(cs, relabelled);
                 const ChangeSetDev dcs = upload_change_set(h, cs);
                 zero_scalar(h, S_NSEL);
-                launch_rebalance_changes_ranked(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, counters, s->sel.as<uint32_t>(),
-                                                h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                if (spread)
+                    launch_rebalance_changes_spread(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, h->spread_tab, counters,
+                                                    s->sel.as<uint32_t>(), h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+                else
+                    launch_rebalance_changes_ranked(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, counters, s->sel.as<uint32_t>(),
+                                                    h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
                 const uint64_t n_sel = read_scalar(h, S_NSEL);
                 if (n_sel) {   // S1: the selected objects' lists computed afresh over the live set, scattered back
                     h->s_keys2.ensure(n_sel * 8, h->stream);
                     h->s_idx.ensure(n_sel * R * 4, h->stream);
                     launch_gather_keys(h->L(), s->keys.as<uint64_t>(), s->sel.as<uint32_t>(), n_sel, h->s_keys2.as<uint64_t>(), nullptr, nullptr);
-                    launch_assign_hrw_ranked(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, R, h->s_idx.as<uint32_t>());
+                    if (spread) launch_assign_hrw_spread(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, h->spread_tab, R, h->s_idx.as<uint32_t>());
+                    else launch_assign_hrw_ranked(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, R, h->s_idx.as<uint32_t>());
                     launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel, R, lists, d_idx, counters, h->tabs.tab.n_total,
                                           h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
                 }
@@ -1939,6 +2014,7 @@ rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *
             moved = read_scalar(h, S_MOVED);
             changed = read_scalar(h, S_CHANGED);
         }
+        if (spread) snapshot_labels(s);
         if (out_moved) *out_moved = moved;
         if (out_changed) *out_changed = changed;
     });

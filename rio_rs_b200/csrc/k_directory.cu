@@ -4,6 +4,8 @@
 #include "kernels.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
+#include "k_spread_changes.cuh"
+#include "k_rank_common.cuh"
 #include "spec.cuh"
 #include "bounded_tail.cuh"
 
@@ -597,15 +599,27 @@ __device__ __forceinline__ void rank_insert(uint64_t (&gs)[R], uint32_t (&gu)[R]
     }
 }
 
+// The same for a failure-domain list (DESIGN.md 3.13): node j of dense domain d, inserted with the domain-aware rule of 3.12.
+template <int R>
+__device__ __forceinline__ void spread_rank_insert(uint64_t (&gs)[R], uint32_t (&gu)[R], uint32_t (&gj)[R], uint32_t (&gd)[R], uint32_t u, uint32_t r,
+                                                   uint32_t j, uint32_t d) {
+    const uint64_t s = (uint64_t)elog(u) * r;
+    if (!cand_better(s, u, j, gs[R - 1], gu[R - 1], gj[R - 1])) return;
+    spread_insert<R>(gs, gu, gj, gd, s, u, j, d);
+}
+
 // Flat policy, 8 + 4R B/object: S1 objects (a list member in REPLACE or past the table) are appended to sel; an S2 list becomes the
 // first R of L u CANDIDATES.  When no member of L is a candidate and L is full, its order is unchanged and a candidate enters only by
 // beating L's last member: one pair hash per candidate, behind challenger_wins's clz bracket.  Only then, or when a member gained
 // weight or L is short, is every member and candidate scored and merged.  The trip loop is block-uniform, so the S1 append can ballot.
-template <int R, bool SMEM>
+// SPREAD (DESIGN.md 3.13): the lists are failure-domain lists and the merge keeps the first R domain representatives, with one dense
+// domain id per scored node read from ndom (n_total x u32) through the read-only path; the gate above is exact for them as well.  The
+// extra argument comes last, so the plain instantiations keep their code.
+template <int R, bool SMEM, bool SPREAD>
 __global__ void __launch_bounds__(256)
 k_rebalance_changes_ranked(const uint64_t *__restrict__ keys, uint32_t *__restrict__ lists, uint32_t *__restrict__ idx, uint64_t n, NodeTabDev tab,
                            ChangeSetDev cs_in, uint32_t *__restrict__ counters, uint32_t *__restrict__ sel, unsigned long long *nsel,
-                           unsigned long long *moved, unsigned long long *changed) {
+                           unsigned long long *moved, unsigned long long *changed, const uint32_t *__restrict__ ndom) {
     const ChangeSetDev cs = stage_changes<SMEM>(cs_in, tab.n_total);
     const uint4 *by_idx = stage_by_idx<SMEM>(tab);
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
@@ -641,14 +655,15 @@ k_rebalance_changes_ranked(const uint64_t *__restrict__ keys, uint32_t *__restri
                 }
                 if (merge) {
                     uint64_t gs[R];
-                    uint32_t gu[R], gj[R];
+                    uint32_t gu[R], gj[R], gd[R];
 #pragma unroll
-                    for (int x = 0; x < R; x++) { gs[x] = ~0ull; gu[x] = 0; gj[x] = kNone; }
+                    for (int x = 0; x < R; x++) { gs[x] = ~0ull; gu[x] = 0; gj[x] = kNone; gd[x] = kNone; }
 #pragma unroll
                     for (int x = 0; x < R; x++) {
                         if (l[x] == kNone) continue;
                         const uint4 r = by_idx[l[x]];
-                        rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, l[x]);
+                        if (SPREAD) spread_rank_insert<R>(gs, gu, gj, gd, pair_hash(o, r.x, r.z, r.w), r.y, l[x], __ldg(ndom + l[x]));
+                        else rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, l[x]);
                     }
                     for (uint32_t q = 0; q < cs.n_cand; q++) {
                         const uint32_t j = cs.cand[q];
@@ -657,7 +672,8 @@ k_rebalance_changes_ranked(const uint64_t *__restrict__ keys, uint32_t *__restri
                         for (int x = 0; x < R; x++) in_l |= l[x] == j;
                         if (in_l) continue;   // a member that gained weight counts once
                         const uint4 r = by_idx[j];
-                        rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, j);
+                        if (SPREAD) spread_rank_insert<R>(gs, gu, gj, gd, pair_hash(o, r.x, r.z, r.w), r.y, j, __ldg(ndom + j));
+                        else rank_insert<R>(gs, gu, gj, pair_hash(o, r.x, r.z, r.w), r.y, j);
                     }
                     bool ch = false;
 #pragma unroll
@@ -966,18 +982,36 @@ void launch_count_changed(const Launch &L, const uint32_t *d_idx, const uint32_t
     k_count_changed<<<grid_for(n_sel, 256, L.sm_count, 8), 256, 0, L.stream>>>(d_idx, d_sel, d_sel_old, n_sel, d_moved);
     RIO_COUNT_LAUNCH(L);
 }
-template <int R>
+// The spread form stages what the ranked one does and reads the 4 B/node domain ids through the read-only path: they are touched
+// only on the merge path, once per scored node, so the 6144-node staging threshold and its shared-memory size stay as they are.
+template <int R, bool SPREAD = false>
 static void rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
                                      const ChangeSetDev &cs, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel, unsigned long long *d_moved,
-                                     unsigned long long *d_changed) {
+                                     unsigned long long *d_changed, const uint32_t *d_ndom = nullptr) {
     const size_t smem = changes_smem(tab, cs);
     const int grid = grid_for(n, 256, L.sm_count, changes_ctas_per_sm(smem));
     if (smem) {
-        cudaFuncSetAttribute(k_rebalance_changes_ranked<R, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChangesMaxSmem);
-        k_rebalance_changes_ranked<R, true><<<grid, 256, smem, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed);
+        cudaFuncSetAttribute(k_rebalance_changes_ranked<R, true, SPREAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, kChangesMaxSmem);
+        k_rebalance_changes_ranked<R, true, SPREAD><<<grid, 256, smem, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed,
+                                                                                  d_ndom);
     } else {
-        k_rebalance_changes_ranked<R, false><<<grid, 256, 0, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed);
+        k_rebalance_changes_ranked<R, false, SPREAD><<<grid, 256, 0, L.stream>>>(d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed,
+                                                                                d_ndom);
     }
+}
+template <int R>
+static void rebalance_changes_spread(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
+                                     const ChangeSetDev &cs, const uint32_t *d_ndom, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel,
+                                     unsigned long long *d_moved, unsigned long long *d_changed) {
+    rebalance_changes_ranked<R, true>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed, d_ndom);
+}
+void launch_rebalance_changes_spread(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t ranks, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
+                                     const ChangeSetDev &cs, const SpreadTabDev &sp, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel,
+                                     unsigned long long *d_moved, unsigned long long *d_changed) {
+    if (!n) return;
+    const uint32_t *d_ndom = reinterpret_cast<const uint32_t *>(sp.base + sp.o_ndom);
+    RIO_RANK_CASES(rebalance_changes_spread, L, d_keys, d_lists, d_idx, n, tab, cs, d_ndom, d_counters, d_sel, d_nsel, d_moved, d_changed)
+    RIO_COUNT_LAUNCH(L);
 }
 void launch_rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t ranks, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
                                      const ChangeSetDev &cs, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel, unsigned long long *d_moved,

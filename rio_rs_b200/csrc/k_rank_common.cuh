@@ -38,6 +38,36 @@ __device__ __forceinline__ bool contest_left_exact(uint32_t v, unsigned long lon
     return phi < qhi || (phi == qhi && plo <= qlo);
 }
 
+// Domain-aware insert of a failure-domain list (DESIGN.md 3.12), best first under the order (E(u)*r, ~u, j) of cand_better, for a
+// candidate the caller has already found better than the last entry.  A listed entry of the same domain that is better drops the
+// candidate; otherwise the shift stops at the same-domain entry it replaces, if there is one.  Dense domain ids: no live node has kNone.
+template <int R>
+__device__ __forceinline__ void spread_insert(uint64_t (&gs)[R], uint32_t (&gu)[R], uint32_t (&gj)[R], uint32_t (&gd)[R], uint64_t s, uint32_t u,
+                                              uint32_t j, uint32_t d) {
+    bool keep = true;
+#pragma unroll
+    for (int y = 0; y < R; y++) keep &= !(gd[y] == d && cand_better(gs[y], gu[y], gj[y], s, u, j));
+    if (!keep) return;
+    const uint32_t dc = d;
+    bool go = true;
+#pragma unroll
+    for (int y = 0; y < R; y++) {
+        const bool sw = go && cand_better(s, u, j, gs[y], gu[y], gj[y]);
+        const uint64_t ts = gs[y]; const uint32_t tu = gu[y], tj = gj[y], td = gd[y];
+        gs[y] = sw ? s : ts; gu[y] = sw ? u : tu; gj[y] = sw ? j : tj; gd[y] = sw ? d : td;
+        s = sw ? ts : s; u = sw ? tu : u; j = sw ? tj : j; d = sw ? td : d;
+        go = go && !(sw && td == dc);
+    }
+}
+
+// Compare mode of the HRW2 walks (DESIGN.md 3.11, 3.13): the output holds the stored lists of a resident set.  Each walk is compared
+// with the stored row, only changed rows are written, and the set's primary index and counters follow column 0.
+struct RankedCmp {
+    uint32_t *idx, *counters;
+    uint32_t n_total;
+    unsigned long long *moved, *changed;
+};
+
 // smem_budget: the most dynamic shared memory the including file's launchers give the kernel.  attr_set: one flag per device for THIS
 // kernel instantiation (the attribute call costs ~1 us of host time per launch otherwise)
 template <class K>

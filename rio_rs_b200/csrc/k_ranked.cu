@@ -77,13 +77,7 @@ k_assign_hrw_ranked(const uint64_t *__restrict__ keys, uint64_t n, NodeTabDev ta
 // ---- HRW2 ----------------------------------------------------------------------------------------------------------------
 // Compare mode (CMP, DESIGN.md 3.11): out_idx holds the stored lists of a resident set.  Each walk is compared with the stored row,
 // only changed rows are written, and the set's primary index and counters follow column 0.  The extra argument comes last, so the
-// plain instantiations keep their parameter layout and code.
-struct RankedCmp {
-    uint32_t *idx, *counters;
-    uint32_t n_total;
-    unsigned long long *moved, *changed;
-};
-
+// plain instantiations keep their parameter layout and code.  RankedCmp is in k_rank_common.cuh.
 template <int R, bool SMEM, bool CMP>
 __global__ void __launch_bounds__(kRankThreads)
 k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, TrieRankDev rk, const __grid_constant__ LevelConsts lc,

@@ -11,6 +11,7 @@
 //     and two prefix differences give the excluded weight on each side of the exact contest of k_assign_trie_ranked.
 #include "k_rank_common.cuh"
 #include "k_spread.cuh"
+#include "k_spread_changes.cuh"
 #include "k_ranked.cuh"
 #include "spec.cuh"
 
@@ -77,6 +78,7 @@ k_assign_hrw_spread(const uint64_t *__restrict__ keys, uint64_t n, NodeTabDev ta
                 uint32_t u = (uint32_t)(ck[x] >> 32), j = ~(uint32_t)ck[x], d = cd[x];
                 uint64_t s = (uint64_t)elog(u) * cr.invw;
                 if (!cand_better(s, u, j, gs[R - 1], gu[R - 1], gj[R - 1])) break;   // the class's later candidates rank lower still
+                // spread_insert of k_rank_common.cuh, written out: called here it changes this kernel's register allocation at R = 1
                 bool keep = true;
 #pragma unroll
                 for (int y = 0; y < R; y++) keep &= !(gd[y] == d && cand_better(gs[y], gu[y], gj[y], s, u, j));
@@ -100,10 +102,14 @@ k_assign_hrw_spread(const uint64_t *__restrict__ keys, uint64_t n, NodeTabDev ta
 }
 
 // ---- HRW2 ----------------------------------------------------------------------------------------------------------------
-template <int R, bool SMEM>
-__global__ void __launch_bounds__(kRankThreads)
+// Compare mode (CMP, DESIGN.md 3.13): out_idx holds the stored lists of a spread resident set, written back only where the walk
+// differs, as in the compare mode of k_assign_trie_ranked.  The extra argument comes last, so the plain instantiations keep their code.
+// The compare instantiations ask for one CTA per SM as their occupancy floor: without that hint ptxas spills at R = 6 to stay at 64
+// registers; with it R = 6 takes 66 and nothing spills (the plain ones have no such hint, as before).
+template <int R, bool SMEM, bool CMP>
+__global__ void __launch_bounds__(kRankThreads, CMP ? 1 : 0)
 k_assign_trie_spread(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, SpreadTabDev sp, const __grid_constant__ LevelConsts lc,
-                     uint32_t *__restrict__ out_idx) {
+                     uint32_t *__restrict__ out_idx, const RankedCmp cmp) {
     extern __shared__ __align__(16) unsigned char smem_spread[];
     const unsigned char *blob = reinterpret_cast<const unsigned char *>(t.blob);
     const unsigned char *side = sp.base;
@@ -124,6 +130,7 @@ k_assign_trie_spread(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, S
     const uint32_t *mb = reinterpret_cast<const uint32_t *>(sp.base + sp.o_mb);
     const uint32_t *dstart = reinterpret_cast<const uint32_t *>(sp.base + sp.o_dstart);
     const uint32_t bits = t.bits;
+    uint32_t n_moved = 0, n_changed = 0;   // compare mode only (a thread walks far fewer than 2^32 objects)
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         const ObjHash o = obj_hash(__ldg(keys + i));
         uint32_t res[R], xd[R];   // ranks so far: node index, its dense domain
@@ -208,8 +215,34 @@ k_assign_trie_spread(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, S
             if (r + 1 < R && nid != kNone) xd[r] = __ldg(ndom + nid);
         }
         uint32_t *dst = out_idx + i * R;
+        if (CMP) {
+            bool changed = false;
 #pragma unroll
-        for (int r = 0; r < R; r++) dst[r] = res[r];
+            for (int r = 0; r < R; r++) changed |= dst[r] != res[r];
+            if (changed) {
+                const uint32_t old0 = dst[0];
+#pragma unroll
+                for (int r = 0; r < R; r++) dst[r] = res[r];
+                n_changed++;
+                if (old0 != res[0]) {
+                    cmp.idx[i] = res[0];
+                    n_moved++;
+                    if (old0 < cmp.n_total) atomicSub(&cmp.counters[old0], 1u);
+                    if (res[0] < cmp.n_total) atomicAdd(&cmp.counters[res[0]], 1u);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int r = 0; r < R; r++) dst[r] = res[r];
+        }
+    }
+    if (CMP) {   // every thread of the block gets here: one atomic per warp and counter
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) { n_moved += __shfl_xor_sync(0xFFFFFFFFu, n_moved, o); n_changed += __shfl_xor_sync(0xFFFFFFFFu, n_changed, o); }
+        if ((threadIdx.x & 31) == 0) {
+            if (n_moved) atomicAdd(cmp.moved, (unsigned long long)n_moved);
+            if (n_changed) atomicAdd(cmp.changed, (unsigned long long)n_changed);
+        }
     }
 }
 
@@ -228,19 +261,23 @@ void hrw_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeT
     }
 }
 
-template <int R>
-void trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t *d_out) {
+template <int R, bool CMP = false>
+void trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t *d_out, const RankedCmp &cmp = {}) {
     static const LevelConsts lc = level_consts();
     const size_t smem = (size_t)t.blob_bytes + sp.o_ndom;
     if (smem <= kSpreadSmemBudget) {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_spread<R, true>, smem, kSpreadSmemBudget, n, attr_set);
-        k_assign_trie_spread<R, true><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, sp, lc, d_out);
+        const int grid = ranked_grid(L, k_assign_trie_spread<R, true, CMP>, smem, kSpreadSmemBudget, n, attr_set);
+        k_assign_trie_spread<R, true, CMP><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, sp, lc, d_out, cmp);
     } else {
         static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_spread<R, false>, 0, kSpreadSmemBudget, n, attr_set);
-        k_assign_trie_spread<R, false><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, sp, lc, d_out);
+        const int grid = ranked_grid(L, k_assign_trie_spread<R, false, CMP>, 0, kSpreadSmemBudget, n, attr_set);
+        k_assign_trie_spread<R, false, CMP><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, sp, lc, d_out, cmp);
     }
+}
+template <int R>
+void trie_spread_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t *d_lists, const RankedCmp &cmp) {
+    trie_spread<R, true>(L, d_keys, n, t, sp, d_lists, cmp);
 }
 
 }  // namespace
@@ -256,6 +293,14 @@ void launch_assign_trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t
                                uint32_t *d_out_idx) {
     if (!n) return;
     RIO_RANK_CASES(trie_spread, L, d_keys, n, t, sp, d_out_idx)
+    if (L.launch_counter) ++*L.launch_counter;
+}
+
+void launch_reassign_trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t ranks, uint32_t *d_lists,
+                                 uint32_t *d_idx, uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {
+    if (!n) return;
+    const RankedCmp cmp{d_idx, d_counters, n_total, d_moved, d_changed};
+    RIO_RANK_CASES(trie_spread_cmp, L, d_keys, n, t, sp, d_lists, cmp)
     if (L.launch_counter) ++*L.launch_counter;
 }
 

@@ -575,6 +575,12 @@ class ObjectSet:
         self._ck(self.L.rio_cuda_set_assign_ranked(self.s, ranks))
         self._ranks = int(ranks)
 
+    def assign_ranked_spread(self, ranks):
+        """Each key's first `ranks` nodes in distinct failure domains, kept in the set (DESIGN.md 3.13), with the labels they were
+        computed under.  read_ranked reads them and rebalance_changes_ranked keeps them current, relabels since the last call included."""
+        self._ck(self.L.rio_cuda_set_assign_ranked_spread(self.s, ranks))
+        self._ranks = int(ranks)
+
     def read_ranked(self, first=0, n=None):
         """Rows [first, first + n) of the ranked lists -> (n, ranks) uint32, RIO_NONE past the live set."""
         if n is None:
