@@ -640,18 +640,29 @@ void run_assign_spread(rio_placement *h, const uint64_t *d_keys, uint64_t n, uin
     else launch_assign_hrw_spread(h->L(), d_keys, n, h->tabs.tab, h->spread_tab, ranks, d_out_idx);
 }
 
-// affinity dispatch: tensor-core (wgmma) kernel for K == 16 (unless RIO_AFFINITY_VARIANT=ffma or the node set does not fit), else CUDA cores
-void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d_out_idx, float *d_out_cost, uint32_t *d_counters) {
-    if (!n) return;
+// affinity dispatch: no live node fills the output with NONE; the tensor-core (wgmma) kernel for K == 16 (unless
+// RIO_AFFINITY_VARIANT=ffma or the node set does not fit); else the CUDA cores
+enum class AffinityPath { kNoLiveNode, kTensorCores, kCudaCores };
+AffinityPath affinity_path(const rio_placement *h) {
     const char *v = getenv("RIO_AFFINITY_VARIANT");
     const bool want_umma = !(v && v[0] == 'f');
-    if (!h->aff_live && h->K == 16 && h->tabs.tab.n_live == 0) { launch_fill_u32(h->L(), d_out_idx, n, kNone); return; }
-    if (want_umma && h->K == 16 && h->aff_live && h->aff_pad <= affinity_umma_max_nodes()) {
-        CUDA_TRY(launch_assign_affinity_umma(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(), h->aff_live, h->aff_pad,
-                                             h->tabs.tab.n_total, d_out_idx, d_out_cost, d_counters));
-        return;
+    if (!h->aff_live && h->K == 16 && h->tabs.tab.n_live == 0) return AffinityPath::kNoLiveNode;
+    if (want_umma && h->K == 16 && h->aff_live && h->aff_pad <= affinity_umma_max_nodes()) return AffinityPath::kTensorCores;
+    return AffinityPath::kCudaCores;
+}
+
+void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d_out_idx, float *d_out_cost, uint32_t *d_counters) {
+    if (!n) return;
+    switch (affinity_path(h)) {
+        case AffinityPath::kNoLiveNode: launch_fill_u32(h->L(), d_out_idx, n, kNone); break;
+        case AffinityPath::kTensorCores:
+            CUDA_TRY(launch_assign_affinity_umma(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(), h->aff_live,
+                                                 h->aff_pad, h->tabs.tab.n_total, d_out_idx, d_out_cost, d_counters));
+            break;
+        case AffinityPath::kCudaCores:
+            launch_assign_affinity(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, d_out_idx, d_out_cost, d_counters);
+            break;
     }
-    launch_assign_affinity(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, d_out_idx, d_out_cost, d_counters);
 }
 
 // each object's `ranks` lowest-cost live nodes (DESIGN.md 3.9), on the path run_affinity takes for the same handle and environment,
@@ -659,16 +670,30 @@ void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d
 void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
     if (!launch_assign_affinity_ranked || !launch_assign_affinity_umma_ranked)
         throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked affinity kernels (k_affinity_umma.cu / k_assign.cu are not linked)"};
-    const char *v = getenv("RIO_AFFINITY_VARIANT");
-    const bool want_umma = !(v && v[0] == 'f');
-    if (!h->aff_live && h->K == 16 && h->tabs.tab.n_live == 0) { launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); return; }
-    if (want_umma && h->K == 16 && h->aff_live && h->aff_pad <= affinity_umma_max_nodes()) {
-        h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
-        CUDA_TRY(launch_assign_affinity_umma_ranked(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(), h->aff_live,
-                                                    h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
-        return;
+    switch (affinity_path(h)) {
+        case AffinityPath::kNoLiveNode: launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); break;
+        case AffinityPath::kTensorCores:
+            h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
+            CUDA_TRY(launch_assign_affinity_umma_ranked(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
+                                                        h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
+            break;
+        case AffinityPath::kCudaCores:
+            launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
+            break;
     }
-    launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
+}
+
+// The host-buffer form of a ranked call: in_n elements from `in` into d_in, run(d_in, h->s_idx) on the device, the n x ranks lists
+// back into out_idx, and the stream synchronised
+template <class T, class F>
+void ranked_from_host(rio_placement *h, DevBuf &d_in, const T *in, size_t in_n, size_t n, uint32_t ranks, uint32_t *out_idx, F &&run) {
+    cudaStream_t st = h->stream;
+    d_in.ensure(in_n * sizeof(T), st);
+    h->s_idx.ensure(n * ranks * 4, st);
+    CUDA_TRY(cudaMemcpyAsync(d_in.p, in, in_n * sizeof(T), cudaMemcpyHostToDevice, st));
+    run(d_in.as<const T>(), h->s_idx.as<uint32_t>());
+    CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
 }
 
 uint32_t capacity_of(uint64_t n_total, uint32_t w, uint64_t w_sum, uint32_t num, uint32_t den) {
@@ -939,6 +964,12 @@ void set_ensure_counters(rio_objset *s) {
         s->counters_alt.ensure(nb.bytes, h->stream);
         s->alt_zero = false;
     }
+}
+
+// every per-node counter of the set to 0, on the handle's stream, before a pass rebuilds them
+void set_zero_counters(rio_objset *s) {
+    rio_placement *h = s->h;
+    CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
 }
 
 }  // namespace
@@ -1363,13 +1394,7 @@ rio_status rio_cuda_assign_ranked_batch(rio_placement *h, const uint64_t *keys, 
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(keys && out_idx, "null buffer");
-        cudaStream_t st = h->stream;
-        h->s_keys.ensure(n * 8, st);
-        h->s_idx.ensure(n * ranks * 4, st);
-        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
-        run_assign_ranked(h, h->s_keys.as<uint64_t>(), n, ranks, h->s_idx.as<uint32_t>());
-        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        ranked_from_host(h, h->s_keys, keys, n, n, ranks, out_idx, [&](const uint64_t *d_keys, uint32_t *d_out) { run_assign_ranked(h, d_keys, n, ranks, d_out); });
     });
 }
 
@@ -1389,13 +1414,7 @@ rio_status rio_cuda_assign_ranked_spread_batch(rio_placement *h, const uint64_t 
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(keys && out_idx, "null buffer");
-        cudaStream_t st = h->stream;
-        h->s_keys.ensure(n * 8, st);
-        h->s_idx.ensure(n * ranks * 4, st);
-        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
-        run_assign_spread(h, h->s_keys.as<uint64_t>(), n, ranks, h->s_idx.as<uint32_t>());
-        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        ranked_from_host(h, h->s_keys, keys, n, n, ranks, out_idx, [&](const uint64_t *d_keys, uint32_t *d_out) { run_assign_spread(h, d_keys, n, ranks, d_out); });
     });
 }
 
@@ -1418,13 +1437,8 @@ rio_status rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *
         REQUIRE(h->K > 0, "assign with object features needs node features");
         REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
         ensure_tab(h);
-        cudaStream_t st = h->stream;
-        h->s_feats.ensure(n * h->K * 4, st);
-        h->s_idx.ensure(n * ranks * 4, st);
-        CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, obj_feats, n * h->K * 4, cudaMemcpyHostToDevice, st));
-        run_affinity_ranked(h, h->s_feats.as<float>(), n, ranks, h->s_idx.as<uint32_t>());
-        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
+        ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
+                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_ranked(h, d_feats, n, ranks, d_out); });
     });
 }
 
@@ -1750,7 +1764,7 @@ rio_status rio_cuda_set_assign(rio_objset *s, uint32_t use_affinity) {
         s->drop_lists();
         ensure_tab(h);
         set_ensure_counters(s);
-        CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+        set_zero_counters(s);
         if (use_affinity) {
             REQUIRE(s->K > 0 && s->K == h->K, "set features / node features missing or of different K");
             run_affinity(h, s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), nullptr, s->counters.as<uint32_t>());
@@ -1821,7 +1835,7 @@ rio_status rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, u
             if (event == RIO_EV_JOIN) REQUIRE(h->nodes[idx].live(), "JOIN of a node that is not live");
             else REQUIRE(!h->nodes[idx].live(), "LEAVE of a node that is still live (deactivate it first)");
             // one streaming pass: walk every key again, write only the indices that changed, rebuild the counters
-            CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+            set_zero_counters(s);
             launch_reassign_trie(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), h->tabs.tab.n_total, h->d_scalars + S_MOVED);
             moved = read_scalar(h, S_MOVED);
         } else if (event == RIO_EV_JOIN) {
@@ -1853,7 +1867,7 @@ rio_status rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, co
             set_ensure_counters(s);
             zero_scalar(h, S_MOVED);
             if (h->solver == RIO_SOLVER_HRW2) {   // one re-walk of every key, counters rebuilt, as rio_cuda_set_rebalance does
-                CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+                set_zero_counters(s);
                 launch_reassign_trie(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), h->tabs.tab.n_total,
                                      h->d_scalars + S_MOVED);
             } else {
@@ -1924,7 +1938,7 @@ void set_assign_lists(rio_objset *s, uint32_t ranks, bool spread) {
     if (spread) run_assign_spread(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
     else run_assign_ranked(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
     launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
-    CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
+    set_zero_counters(s);
     launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
     s->assigned = true;
     s->ranks = ranks;

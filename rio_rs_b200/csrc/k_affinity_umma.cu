@@ -526,8 +526,6 @@ k_affinity_resolve_ranked(const float *__restrict__ fobj, uint64_t n, const floa
 
 }  // namespace
 
-#define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
-
 // development hook: device buffer of 16 u64 per CTA that receives the tensor-core kernel's setup and total cycle counts
 static unsigned long long *g_umma_timing = nullptr;
 void affinity_umma_set_timing_buffer(unsigned long long *d) { g_umma_timing = d; }

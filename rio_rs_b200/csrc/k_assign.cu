@@ -567,8 +567,6 @@ static int assign_variant() {
     return (e && e[0] == '1') ? 1 : 2;
 }
 
-#define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
-
 // Objects one full wave of the default rendezvous launch covers (persistent CTAs x objects per tile): host code that
 // pipelines chunks sizes them in whole waves so that no chunk ends on a partially filled wave.
 constexpr int kV2DefaultTune = 532;   // 5 objects per thread, 3 CTAs per SM, 32-node straight-line groups

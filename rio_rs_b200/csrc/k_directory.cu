@@ -13,8 +13,6 @@ namespace rio {
 
 namespace {
 
-#define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
-
 inline int grid_for(uint64_t work_items, int threads, int sm_count, int blocks_per_sm) {
     uint64_t blocks = (work_items + threads - 1) / threads;
     uint64_t cap = (uint64_t)sm_count * blocks_per_sm;
@@ -999,36 +997,22 @@ static void rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, ui
                                                                                 d_ndom);
     }
 }
-template <int R>
-static void rebalance_changes_spread(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
-                                     const ChangeSetDev &cs, const uint32_t *d_ndom, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel,
-                                     unsigned long long *d_moved, unsigned long long *d_changed) {
-    rebalance_changes_ranked<R, true>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed, d_ndom);
-}
 void launch_rebalance_changes_spread(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t ranks, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
                                      const ChangeSetDev &cs, const SpreadTabDev &sp, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel,
                                      unsigned long long *d_moved, unsigned long long *d_changed) {
     if (!n) return;
     const uint32_t *d_ndom = reinterpret_cast<const uint32_t *>(sp.base + sp.o_ndom);
-    RIO_RANK_CASES(rebalance_changes_spread, L, d_keys, d_lists, d_idx, n, tab, cs, d_ndom, d_counters, d_sel, d_nsel, d_moved, d_changed)
-    RIO_COUNT_LAUNCH(L);
+    if (with_ranks(ranks, [&](auto r) {
+            rebalance_changes_ranked<r, true>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed, d_ndom);
+        }))
+        RIO_COUNT_LAUNCH(L);
 }
 void launch_rebalance_changes_ranked(const Launch &L, const uint64_t *d_keys, uint32_t *d_lists, uint32_t ranks, uint32_t *d_idx, uint64_t n, const NodeTabDev &tab,
                                      const ChangeSetDev &cs, uint32_t *d_counters, uint32_t *d_sel, unsigned long long *d_nsel, unsigned long long *d_moved,
                                      unsigned long long *d_changed) {
     if (!n) return;
-    switch (ranks) {
-        case 1: rebalance_changes_ranked<1>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 2: rebalance_changes_ranked<2>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 3: rebalance_changes_ranked<3>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 4: rebalance_changes_ranked<4>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 5: rebalance_changes_ranked<5>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 6: rebalance_changes_ranked<6>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 7: rebalance_changes_ranked<7>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        case 8: rebalance_changes_ranked<8>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); break;
-        default: return;
-    }
-    RIO_COUNT_LAUNCH(L);
+    if (with_ranks(ranks, [&](auto r) { rebalance_changes_ranked<r>(L, d_keys, d_lists, d_idx, n, tab, cs, d_counters, d_sel, d_nsel, d_moved, d_changed); }))
+        RIO_COUNT_LAUNCH(L);
 }
 void launch_scatter_ranked(const Launch &L, const uint32_t *d_fresh, const uint32_t *d_sel, uint64_t n_sel, uint32_t ranks, uint32_t *d_lists, uint32_t *d_idx,
                            uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {

@@ -1,8 +1,11 @@
-// k_rank_common.cuh -- launch shape, shared-memory staging and the exact HRW2 contest of the ranked walks (k_ranked.cu, k_spread.cu).
+// k_rank_common.cuh -- launch shape, shared-memory staging, the exact HRW2 contest, the compare-mode epilogue and the rank dispatch of
+// the ranked walks (k_ranked.cu, k_spread.cu) and the ranked change-set passes (k_directory.cu).
 // Included by .cu files only: everything is internal to the including translation unit.
 #pragma once
 #include "kernels.cuh"
 #include "spec.cuh"
+
+#include <type_traits>
 
 namespace rio {
 
@@ -68,6 +71,45 @@ struct RankedCmp {
     unsigned long long *moved, *changed;
 };
 
+// Stores object i's finished row res at dst.  Compare mode counts a changed row in n_changed and a changed column 0 in n_moved.
+template <int R, bool CMP>
+__device__ __forceinline__ void ranked_store(uint32_t *dst, const uint32_t (&res)[R], uint64_t i, const RankedCmp &cmp, uint32_t &n_moved,
+                                             uint32_t &n_changed) {
+    if (CMP) {
+        bool changed = false;
+#pragma unroll
+        for (int r = 0; r < R; r++) changed |= dst[r] != res[r];
+        if (changed) {
+            const uint32_t old0 = dst[0];
+#pragma unroll
+            for (int r = 0; r < R; r++) dst[r] = res[r];
+            n_changed++;
+            if (old0 != res[0]) {
+                cmp.idx[i] = res[0];
+                n_moved++;
+                if (old0 < cmp.n_total) atomicSub(&cmp.counters[old0], 1u);
+                if (res[0] < cmp.n_total) atomicAdd(&cmp.counters[res[0]], 1u);
+            }
+        }
+    } else {
+#pragma unroll
+        for (int r = 0; r < R; r++) dst[r] = res[r];
+    }
+}
+
+// The end of a compare-mode kernel: every thread of the block gets here; one atomic per warp and counter.
+template <bool CMP>
+__device__ __forceinline__ void ranked_flush(const RankedCmp &cmp, uint32_t n_moved, uint32_t n_changed) {
+    if (CMP) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) { n_moved += __shfl_xor_sync(0xFFFFFFFFu, n_moved, o); n_changed += __shfl_xor_sync(0xFFFFFFFFu, n_changed, o); }
+        if ((threadIdx.x & 31) == 0) {
+            if (n_moved) atomicAdd(cmp.moved, (unsigned long long)n_moved);
+            if (n_changed) atomicAdd(cmp.changed, (unsigned long long)n_changed);
+        }
+    }
+}
+
 // smem_budget: the most dynamic shared memory the including file's launchers give the kernel.  attr_set: one flag per device for THIS
 // kernel instantiation (the attribute call costs ~1 us of host time per launch otherwise)
 template <class K>
@@ -84,11 +126,30 @@ int ranked_grid(const Launch &L, K kern, size_t smem, uint32_t smem_budget, uint
     return (int)(blocks < cap ? blocks : cap);
 }
 
+// Launches kernel K over n objects with kRankThreads threads and smem bytes of dynamic shared memory
+template <auto K, class... A>
+void launch_rank_kernel(const Launch &L, size_t smem, uint32_t smem_budget, uint64_t n, const A &...args) {
+    static bool attr_set[64] = {};
+    const int grid = ranked_grid(L, K, smem, smem_budget, n, attr_set);
+    K<<<grid, kRankThreads, smem, L.stream>>>(args...);
+}
+
+// Calls f(std::integral_constant<int, R>{}) for ranks = R in 1..8 and returns true; any other ranks launches nothing and returns false
+template <class F>
+bool with_ranks(uint32_t ranks, F &&f) {
+    switch (ranks) {
+        case 1: f(std::integral_constant<int, 1>{}); return true;
+        case 2: f(std::integral_constant<int, 2>{}); return true;
+        case 3: f(std::integral_constant<int, 3>{}); return true;
+        case 4: f(std::integral_constant<int, 4>{}); return true;
+        case 5: f(std::integral_constant<int, 5>{}); return true;
+        case 6: f(std::integral_constant<int, 6>{}); return true;
+        case 7: f(std::integral_constant<int, 7>{}); return true;
+        case 8: f(std::integral_constant<int, 8>{}); return true;
+        default: return false;
+    }
+}
+
 }  // namespace
 
 }  // namespace rio
-
-#define RIO_RANK_CASES(F, ...) \
-    switch (ranks) { case 1: F<1>(__VA_ARGS__); break; case 2: F<2>(__VA_ARGS__); break; case 3: F<3>(__VA_ARGS__); break; \
-                     case 4: F<4>(__VA_ARGS__); break; case 5: F<5>(__VA_ARGS__); break; case 6: F<6>(__VA_ARGS__); break; \
-                     case 7: F<7>(__VA_ARGS__); break; case 8: F<8>(__VA_ARGS__); break; default: return; }

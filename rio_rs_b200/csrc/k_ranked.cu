@@ -77,7 +77,8 @@ k_assign_hrw_ranked(const uint64_t *__restrict__ keys, uint64_t n, NodeTabDev ta
 // ---- HRW2 ----------------------------------------------------------------------------------------------------------------
 // Compare mode (CMP, DESIGN.md 3.11): out_idx holds the stored lists of a resident set.  Each walk is compared with the stored row,
 // only changed rows are written, and the set's primary index and counters follow column 0.  The extra argument comes last, so the
-// plain instantiations keep their parameter layout and code.  RankedCmp is in k_rank_common.cuh.
+// plain instantiations keep their parameter layout and code.  RankedCmp and the epilogue (ranked_store, ranked_flush) are in
+// k_rank_common.cuh.
 template <int R, bool SMEM, bool CMP>
 __global__ void __launch_bounds__(kRankThreads)
 k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, TrieRankDev rk, const __grid_constant__ LevelConsts lc,
@@ -167,49 +168,18 @@ k_assign_trie_ranked(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, T
                 xw[r] = nd.y;
             }
         }
-        uint32_t *dst = out_idx + i * R;
-        if (CMP) {
-            bool changed = false;
-#pragma unroll
-            for (int r = 0; r < R; r++) changed |= dst[r] != res[r];
-            if (changed) {
-                const uint32_t old0 = dst[0];
-#pragma unroll
-                for (int r = 0; r < R; r++) dst[r] = res[r];
-                n_changed++;
-                if (old0 != res[0]) {
-                    cmp.idx[i] = res[0];
-                    n_moved++;
-                    if (old0 < cmp.n_total) atomicSub(&cmp.counters[old0], 1u);
-                    if (res[0] < cmp.n_total) atomicAdd(&cmp.counters[res[0]], 1u);
-                }
-            }
-        } else {
-#pragma unroll
-            for (int r = 0; r < R; r++) dst[r] = res[r];
-        }
+        ranked_store<R, CMP>(out_idx + i * R, res, i, cmp, n_moved, n_changed);
     }
-    if (CMP) {   // every thread of the block gets here: one atomic per warp and counter
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { n_moved += __shfl_xor_sync(0xFFFFFFFFu, n_moved, o); n_changed += __shfl_xor_sync(0xFFFFFFFFu, n_changed, o); }
-        if ((threadIdx.x & 31) == 0) {
-            if (n_moved) atomicAdd(cmp.moved, (unsigned long long)n_moved);
-            if (n_changed) atomicAdd(cmp.changed, (unsigned long long)n_changed);
-        }
-    }
+    ranked_flush<CMP>(cmp, n_moved, n_changed);
 }
 
 template <int R>
 void hrw_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeTabDev &tab, uint32_t *d_out) {
     const size_t smem = (size_t)tab.n_live * 16;
     if (smem <= 96u * 1024u) {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, true>, smem, kRankSmemBudget, n, attr_set);
-        k_assign_hrw_ranked<R, true><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, tab, d_out);
+        launch_rank_kernel<k_assign_hrw_ranked<R, true>>(L, smem, kRankSmemBudget, n, d_keys, n, tab, d_out);
     } else {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_ranked<R, false>, 0, kRankSmemBudget, n, attr_set);
-        k_assign_hrw_ranked<R, false><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, tab, d_out);
+        launch_rank_kernel<k_assign_hrw_ranked<R, false>>(L, 0, kRankSmemBudget, n, d_keys, n, tab, d_out);
     }
 }
 
@@ -218,41 +188,30 @@ void trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const Trie
     static const LevelConsts lc = level_consts();
     const size_t smem = (size_t)t.blob_bytes + rk.bytes;
     if (smem <= kRankSmemBudget) {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, true, CMP>, smem, kRankSmemBudget, n, attr_set);
-        k_assign_trie_ranked<R, true, CMP><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
+        launch_rank_kernel<k_assign_trie_ranked<R, true, CMP>>(L, smem, kRankSmemBudget, n, d_keys, n, t, rk, lc, d_out, cmp);
     } else {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_ranked<R, false, CMP>, 0, kRankSmemBudget, n, attr_set);
-        k_assign_trie_ranked<R, false, CMP><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, rk, lc, d_out, cmp);
+        launch_rank_kernel<k_assign_trie_ranked<R, false, CMP>>(L, 0, kRankSmemBudget, n, d_keys, n, t, rk, lc, d_out, cmp);
     }
-}
-template <int R>
-void trie_ranked_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t *d_lists, const RankedCmp &cmp) {
-    trie_ranked<R, true>(L, d_keys, n, t, rk, d_lists, cmp);
 }
 
 }  // namespace
 
 void launch_assign_hrw_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeTabDev &tab, uint32_t ranks, uint32_t *d_out_idx) {
     if (!n) return;
-    RIO_RANK_CASES(hrw_ranked, L, d_keys, n, tab, d_out_idx)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { hrw_ranked<r>(L, d_keys, n, tab, d_out_idx); })) RIO_COUNT_LAUNCH(L);
 }
 
 void launch_assign_trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t ranks,
                                uint32_t *d_out_idx) {
     if (!n) return;
-    RIO_RANK_CASES(trie_ranked, L, d_keys, n, t, rk, d_out_idx)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { trie_ranked<r>(L, d_keys, n, t, rk, d_out_idx); })) RIO_COUNT_LAUNCH(L);
 }
 
 void launch_reassign_trie_ranked(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const TrieRankDev &rk, uint32_t ranks, uint32_t *d_lists,
                                  uint32_t *d_idx, uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {
     if (!n) return;
     const RankedCmp cmp{d_idx, d_counters, n_total, d_moved, d_changed};
-    RIO_RANK_CASES(trie_ranked_cmp, L, d_keys, n, t, rk, d_lists, cmp)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { trie_ranked<r, true>(L, d_keys, n, t, rk, d_lists, cmp); })) RIO_COUNT_LAUNCH(L);
 }
 
 }  // namespace rio

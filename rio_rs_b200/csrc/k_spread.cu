@@ -214,36 +214,9 @@ k_assign_trie_spread(const uint64_t *__restrict__ keys, uint64_t n, TrieDev t, S
             res[r] = nid;
             if (r + 1 < R && nid != kNone) xd[r] = __ldg(ndom + nid);
         }
-        uint32_t *dst = out_idx + i * R;
-        if (CMP) {
-            bool changed = false;
-#pragma unroll
-            for (int r = 0; r < R; r++) changed |= dst[r] != res[r];
-            if (changed) {
-                const uint32_t old0 = dst[0];
-#pragma unroll
-                for (int r = 0; r < R; r++) dst[r] = res[r];
-                n_changed++;
-                if (old0 != res[0]) {
-                    cmp.idx[i] = res[0];
-                    n_moved++;
-                    if (old0 < cmp.n_total) atomicSub(&cmp.counters[old0], 1u);
-                    if (res[0] < cmp.n_total) atomicAdd(&cmp.counters[res[0]], 1u);
-                }
-            }
-        } else {
-#pragma unroll
-            for (int r = 0; r < R; r++) dst[r] = res[r];
-        }
+        ranked_store<R, CMP>(out_idx + i * R, res, i, cmp, n_moved, n_changed);
     }
-    if (CMP) {   // every thread of the block gets here: one atomic per warp and counter
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { n_moved += __shfl_xor_sync(0xFFFFFFFFu, n_moved, o); n_changed += __shfl_xor_sync(0xFFFFFFFFu, n_changed, o); }
-        if ((threadIdx.x & 31) == 0) {
-            if (n_moved) atomicAdd(cmp.moved, (unsigned long long)n_moved);
-            if (n_changed) atomicAdd(cmp.changed, (unsigned long long)n_changed);
-        }
-    }
+    ranked_flush<CMP>(cmp, n_moved, n_changed);
 }
 
 template <int R>
@@ -251,13 +224,9 @@ void hrw_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeT
     const uint32_t *pos_dom = reinterpret_cast<const uint32_t *>(sp.base + sp.trie_bytes);
     const size_t smem = (size_t)tab.n_live * 16 + ((size_t)tab.n_live * 4 + 15) / 16 * 16;
     if (smem <= 96u * 1024u) {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_spread<R, true>, smem, kSpreadSmemBudget, n, attr_set);
-        k_assign_hrw_spread<R, true><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, tab, pos_dom, d_out);
+        launch_rank_kernel<k_assign_hrw_spread<R, true>>(L, smem, kSpreadSmemBudget, n, d_keys, n, tab, pos_dom, d_out);
     } else {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_hrw_spread<R, false>, 0, kSpreadSmemBudget, n, attr_set);
-        k_assign_hrw_spread<R, false><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, tab, pos_dom, d_out);
+        launch_rank_kernel<k_assign_hrw_spread<R, false>>(L, 0, kSpreadSmemBudget, n, d_keys, n, tab, pos_dom, d_out);
     }
 }
 
@@ -266,18 +235,10 @@ void trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const Trie
     static const LevelConsts lc = level_consts();
     const size_t smem = (size_t)t.blob_bytes + sp.o_ndom;
     if (smem <= kSpreadSmemBudget) {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_spread<R, true, CMP>, smem, kSpreadSmemBudget, n, attr_set);
-        k_assign_trie_spread<R, true, CMP><<<grid, kRankThreads, smem, L.stream>>>(d_keys, n, t, sp, lc, d_out, cmp);
+        launch_rank_kernel<k_assign_trie_spread<R, true, CMP>>(L, smem, kSpreadSmemBudget, n, d_keys, n, t, sp, lc, d_out, cmp);
     } else {
-        static bool attr_set[64] = {};
-        const int grid = ranked_grid(L, k_assign_trie_spread<R, false, CMP>, 0, kSpreadSmemBudget, n, attr_set);
-        k_assign_trie_spread<R, false, CMP><<<grid, kRankThreads, 0, L.stream>>>(d_keys, n, t, sp, lc, d_out, cmp);
+        launch_rank_kernel<k_assign_trie_spread<R, false, CMP>>(L, 0, kSpreadSmemBudget, n, d_keys, n, t, sp, lc, d_out, cmp);
     }
-}
-template <int R>
-void trie_spread_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t *d_lists, const RankedCmp &cmp) {
-    trie_spread<R, true>(L, d_keys, n, t, sp, d_lists, cmp);
 }
 
 }  // namespace
@@ -285,23 +246,20 @@ void trie_spread_cmp(const Launch &L, const uint64_t *d_keys, uint64_t n, const 
 void launch_assign_hrw_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const NodeTabDev &tab, const SpreadTabDev &sp, uint32_t ranks,
                               uint32_t *d_out_idx) {
     if (!n) return;
-    RIO_RANK_CASES(hrw_spread, L, d_keys, n, tab, sp, d_out_idx)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { hrw_spread<r>(L, d_keys, n, tab, sp, d_out_idx); })) RIO_COUNT_LAUNCH(L);
 }
 
 void launch_assign_trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t ranks,
                                uint32_t *d_out_idx) {
     if (!n) return;
-    RIO_RANK_CASES(trie_spread, L, d_keys, n, t, sp, d_out_idx)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { trie_spread<r>(L, d_keys, n, t, sp, d_out_idx); })) RIO_COUNT_LAUNCH(L);
 }
 
 void launch_reassign_trie_spread(const Launch &L, const uint64_t *d_keys, uint64_t n, const TrieDev &t, const SpreadTabDev &sp, uint32_t ranks, uint32_t *d_lists,
                                  uint32_t *d_idx, uint32_t *d_counters, uint32_t n_total, unsigned long long *d_moved, unsigned long long *d_changed) {
     if (!n) return;
     const RankedCmp cmp{d_idx, d_counters, n_total, d_moved, d_changed};
-    RIO_RANK_CASES(trie_spread_cmp, L, d_keys, n, t, sp, d_lists, cmp)
-    if (L.launch_counter) ++*L.launch_counter;
+    if (with_ranks(ranks, [&](auto r) { trie_spread<r, true>(L, d_keys, n, t, sp, d_lists, cmp); })) RIO_COUNT_LAUNCH(L);
 }
 
 }  // namespace rio

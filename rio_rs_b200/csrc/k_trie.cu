@@ -19,8 +19,6 @@ namespace rio {
 
 namespace {
 
-#define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
-
 constexpr int kTrieThreads = 256;
 constexpr uint32_t kMaxLevels = 16;          // trie_bits <= 14; the table has two spare entries
 

@@ -58,6 +58,8 @@ struct DirDev {
 };
 
 struct Launch { cudaStream_t stream; int sm_count; uint64_t *launch_counter; int spare_ctas = 0; /* dense walk: leave this many CTA slots of the machine free */ };
+// every launcher counts each kernel it launched (rio_cuda_launch_count)
+#define RIO_COUNT_LAUNCH(L) do { if ((L).launch_counter) ++*(L).launch_counter; } while (0)
 
 // ---- the tail of a bounded-load pass: counter exchange + capacity check (bounded_tail.cuh) ----------------------------------
 struct XchgPeers { uint32_t *win[16]; };
