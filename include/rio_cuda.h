@@ -162,6 +162,13 @@ rio_status  rio_cuda_assign_ranked_spread_batch(rio_placement *h, const uint64_t
  * n x K (K of set_nodes), out_idx n x ranks row-major, RIO_NONE past the live node count.  RIO_ERR_UNKNOWN as for
  * rio_cuda_assign_ranked_batch, and when the handle has no node features. */
 rio_status  rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx);
+/* Ranked placement under the affinity cost across failure domains (DESIGN.md 3.14): rank 1 is exactly what assign_batch with the
+ * same obj_feats returns; rank r is the lowest (cost, node index) over the live set minus every node whose domain is the domain of
+ * one of ranks 1..r-1.  The ranks lie in distinct domains, rank 2 is where the object goes when rank 1's whole domain leaves, and the
+ * entries past the number of distinct live domains are RIO_NONE.  With no labels set the result is rio_cuda_assign_ranked_affinity_batch's.
+ * Output and argument errors as for rio_cuda_assign_ranked_affinity_batch; RIO_ERR_UPSTREAM when the library was built without the
+ * failure-domain affinity kernels. */
+rio_status  rio_cuda_assign_ranked_affinity_spread_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx);
 /* Service::get_or_create_placement for a batch (service.rs:193-254): existing & live => keep; recorded on an
  * inactive node => clean_server(that node) then re-place; none => place.  policy RIO_PLACE_SELF re-places on
  * self_idx (the reference's rule, service.rs:244-252); RIO_PLACE_HRW / RIO_PLACE_HRW2 re-place by the solver. */
@@ -294,6 +301,7 @@ rio_status  rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, 
 rio_status  rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_assign_ranked_spread_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx);
+rio_status  rio_cuda_assign_ranked_affinity_spread_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx);
 rio_status  rio_cuda_lookup_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t *d_out_idx);
 rio_status  rio_cuda_upsert_batch_dev(rio_placement *h, const uint64_t *d_keys, const uint32_t *d_idx, size_t n);
 /* pre-size the directory for n more distinct keys (the _dev upsert cannot grow it mid-stream) */

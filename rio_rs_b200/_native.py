@@ -68,6 +68,8 @@ SIGNATURES = {
     "rio_cuda_assign_ranked_spread_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_affinity_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_affinity_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
+    "rio_cuda_assign_ranked_affinity_spread_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
+    "rio_cuda_assign_ranked_affinity_spread_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_check_address_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp, u64p]),
     "rio_cuda_place_batch": (C.c_int32, [H, vp, sz, C.c_uint32, C.c_uint32, vp]),
     "rio_cuda_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),

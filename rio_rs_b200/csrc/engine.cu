@@ -9,6 +9,7 @@
 #include "kernels.cuh"
 #include "k_ranked.cuh"
 #include "k_affinity_ranked.cuh"
+#include "k_affinity_spread.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -199,6 +200,11 @@ struct rio_placement {
     std::vector<unsigned char> spread_stage;
     SpreadTabDev spread_tab{};
     uint64_t spread_version[2] = {~0ull, ~0ull};   // (tab_version, label_version) the side table belongs to
+    // dense domain ids of the failure-domain affinity lists (DESIGN.md 3.14): n_total per interned index, then aff_pad per compacted
+    // affinity position (the order of d_nidx_map), built on the first such call after a table or label change
+    DevBuf aff_dom;
+    size_t aff_dom_pos = 0;                        // offset of the per-position ids in aff_dom
+    uint64_t aff_dom_version[2] = {~0ull, ~0ull};
     unsigned long long *d_scalars = nullptr;   // S_COUNT u64 + error u32
     unsigned long long *h_scalars = nullptr;   // pinned mirror
 
@@ -566,6 +572,21 @@ void run_assign_ranked(rio_placement *h, const uint64_t *d_keys, uint64_t n, uin
     }
 }
 
+// Dense domain ids of the live nodes per interned index (kNone for the others): one per label shared by live nodes, one per live
+// node labelled RIO_NONE, numbered in node-index order.  Returns the number of domains.
+uint32_t dense_domains(const rio_placement *h, std::vector<uint32_t> &ndom) {
+    ndom.assign(h->nodes.size(), kNone);
+    std::unordered_map<uint32_t, uint32_t> dense;
+    uint32_t n_dom = 0;
+    for (uint32_t j = 0; j < (uint32_t)h->nodes.size(); j++) {
+        const NodeInfo &ni = h->nodes[j];
+        if (!ni.live()) continue;
+        if (ni.domain == RIO_NONE) ndom[j] = n_dom++;
+        else ndom[j] = dense.emplace(ni.domain, n_dom).second ? n_dom++ : dense[ni.domain];
+    }
+    return n_dom;
+}
+
 // The spread walks need the ranked side table plus the live members grouped by domain: dense domain ids (one per label shared by
 // live nodes, one per live node labelled RIO_NONE), the members sorted by (domain, bucket, index) with a running weight, and for the
 // flat kernel the domain of every record in the class-sorted order build_tab gives the table, (inverse weight, node index).
@@ -573,16 +594,13 @@ void ensure_spread_tab(rio_placement *h) {
     if (h->spread_version[0] == h->tab_version && h->spread_version[1] == h->label_version) return;
     const uint32_t n_total = (uint32_t)h->nodes.size();
     std::vector<TrieMember> members;
-    std::vector<uint32_t> live, ndom(n_total, kNone);
-    std::unordered_map<uint32_t, uint32_t> dense;
-    uint32_t n_dom = 0;
+    std::vector<uint32_t> live, ndom;
+    const uint32_t n_dom = dense_domains(h, ndom);
     for (uint32_t j = 0; j < n_total; j++) {
         const NodeInfo &ni = h->nodes[j];
         if (!ni.live()) continue;
         members.push_back(TrieMember{ni.seed, j, ni.weight});
         live.push_back(j);
-        if (ni.domain == RIO_NONE) ndom[j] = n_dom++;
-        else ndom[j] = dense.emplace(ni.domain, n_dom).second ? n_dom++ : dense[ni.domain];
     }
     const TrieBlob blob = build_trie_blob(members, h->trie_bits);
     const uint32_t bits = blob.bits, nb = 1u << bits, n_live = (uint32_t)live.size();
@@ -680,6 +698,46 @@ void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint
         case AffinityPath::kCudaCores:
             launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
             break;
+    }
+}
+
+// The domain ids of the failure-domain affinity lists: without the HRW2 blob ensure_spread_tab builds, so the first call after a
+// relabel costs one pass over the nodes and one small copy
+void ensure_aff_dom(rio_placement *h) {
+    if (h->aff_dom_version[0] == h->tab_version && h->aff_dom_version[1] == h->label_version) return;
+    std::vector<uint32_t> ids;
+    dense_domains(h, ids);
+    const size_t n_total = ids.size();
+    if (h->aff_pad) {   // the live nodes in node-index order, padded with kNone: the compacted positions of ensure_tab
+        ids.reserve(n_total + h->aff_pad);
+        for (size_t j = 0; j < n_total; j++)
+            if (ids[j] != kNone) ids.push_back(ids[j]);
+        ids.resize(n_total + h->aff_pad, kNone);
+    }
+    if (ids.empty()) ids.push_back(kNone);
+    h->aff_dom.ensure(ids.size() * 4, h->stream);
+    CUDA_TRY(cudaMemcpyAsync(h->aff_dom.p, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));   // ids goes out of scope
+    h->aff_dom_pos = n_total;
+    h->aff_dom_version[0] = h->tab_version;
+    h->aff_dom_version[1] = h->label_version;
+}
+
+// each object's `ranks` lowest-cost live nodes in distinct failure domains (DESIGN.md 3.14), on the path run_affinity takes, so that
+// rank 1 is its answer; the tensor-core pair keeps each object's listed column positions in s_idx2 between the two passes
+void run_affinity_spread(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!launch_assign_affinity_spread || !launch_assign_affinity_umma_spread)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no failure-domain affinity kernels (k_affinity_spread.cuh launchers are not linked)"};
+    const AffinityPath path = affinity_path(h);
+    if (path == AffinityPath::kNoLiveNode) { launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); return; }
+    ensure_aff_dom(h);
+    const uint32_t *ndom = h->aff_dom.as<uint32_t>();
+    if (path == AffinityPath::kTensorCores) {
+        h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
+        CUDA_TRY(launch_assign_affinity_umma_spread(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
+                                                    ndom + h->aff_dom_pos, h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
+    } else {
+        launch_assign_affinity_spread(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ndom, ranks, d_out_idx);
     }
 }
 
@@ -1056,7 +1114,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev, &h->spread_dev};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev, &h->spread_dev, &h->aff_dom};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -1451,6 +1509,32 @@ rio_status rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const flo
         REQUIRE(h->K > 0, "assign with object features needs node features");
         ensure_tab(h);
         run_affinity_ranked(h, d_obj_feats, n, ranks, d_out_idx);
+    });
+}
+
+rio_status rio_cuda_assign_ranked_affinity_spread_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(obj_feats && out_idx, "null buffer");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
+        ensure_tab(h);
+        ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
+                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_spread(h, d_feats, n, ranks, d_out); });
+    });
+}
+
+rio_status rio_cuda_assign_ranked_affinity_spread_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        check_ranked_args(n, ranks);
+        if (!n) return;
+        REQUIRE(d_obj_feats && d_out_idx, "null buffer");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        ensure_tab(h);
+        run_affinity_spread(h, d_obj_feats, n, ranks, d_out_idx);
     });
 }
 

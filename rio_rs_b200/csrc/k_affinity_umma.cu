@@ -22,6 +22,7 @@
 // fp32 cost + per-node histogram.
 #include "kernels.cuh"
 #include "k_affinity_ranked.cuh"
+#include "k_affinity_spread.cuh"
 #include "spec.cuh"
 
 #include <cuda_bf16.h>
@@ -524,6 +525,203 @@ k_affinity_resolve_ranked(const float *__restrict__ fobj, uint64_t n, const floa
     }
 }
 
+// ---- failure-domain lists (DESIGN.md 3.14) ----------------------------------------------------------------------------------------
+// A row's list of RT columns (value, position, domain), one per domain, ordered by larger value, then smaller position; empty slots
+// are (-inf, kNone, kNone).
+__device__ __forceinline__ bool col_before(float v, uint32_t p, float w, uint32_t q) { return v > w || (v == w && p < q); }
+
+// Domain-aware insert (the rule of spread_insert, DESIGN.md 3.12) of a column the caller found before the last entry: a listed column
+// of the same domain that comes before it drops it; otherwise it goes in place and the shift stops at the entry of its own domain.
+template <int RT>
+__device__ __forceinline__ void insert_dom(float (&lv)[RT], uint32_t (&lp)[RT], uint32_t (&ld)[RT], float v, uint32_t p, uint32_t d) {
+    bool keep = true;
+#pragma unroll
+    for (int i = 0; i < RT; i++) keep &= !(ld[i] == d && col_before(lv[i], lp[i], v, p));
+    if (!keep) return;
+    const uint32_t dc = d;
+    bool go = true;
+#pragma unroll
+    for (int i = 0; i < RT; i++) {
+        const bool sw = go && col_before(v, p, lv[i], lp[i]);
+        const float tv = lv[i];
+        const uint32_t tp = lp[i], td = ld[i];
+        lv[i] = sw ? v : tv; lp[i] = sw ? p : tp; ld[i] = sw ? d : td;
+        v = sw ? tv : v; p = sw ? tp : p; d = sw ? td : d;
+        go = go && !(sw && td == dc);
+    }
+}
+
+// k_affinity_wgmma_ranked keeping, per row, the best RT domain representatives among the COLUMNS (not groups) in
+// out_idx[row * RT ..], kNone past the live domains.  Node staging, the A fragments and the six-term tiles are k_affinity_wgmma's, so
+// the accumulators are the same bits.  A lane scans its columns in increasing position, so `v > last value` is an exact gate, and the
+// domain id is read (read-only path) on the insert path only.  The four lane lists of a row merge with the same insert (xor 1, 2).
+// The first entry is the row's largest value at its smallest position, so its group is the one k_affinity_wgmma picks.
+template <int NT, int RT, int WG>
+__global__ void __launch_bounds__(128 * WG, 1) k_affinity_wgmma_spread(WgmmaParams P, const uint32_t *__restrict__ pdom) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    unsigned char *sB = smem;
+    const uint32_t b_block_bytes = P.m_pad * 32;
+    for (uint32_t p = threadIdx.x; p < P.m_pad; p += blockDim.x) {
+        float f[16];
+        const float4 *row = reinterpret_cast<const float4 *>(P.fnode_c + (size_t)p * 16);
+#pragma unroll
+        for (int q = 0; q < 4; q++) { const float4 v = __ldg(row + q); f[4 * q] = v.x; f[4 * q + 1] = v.y; f[4 * q + 2] = v.z; f[4 * q + 3] = v.w; }
+        store_row_split(sB, b_block_bytes, P.m_pad * 16, p, f);
+    }
+    fence_proxy_async();
+    __syncthreads();
+
+    const uint32_t wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const uint32_t q = lane & 3, r_in = warp * 16 + (lane >> 2);
+    const uint32_t n_tiles = P.m_pad / NT;
+    const uint64_t n_rb = (P.n + kRows - 1) / kRows, rb_step = (uint64_t)gridDim.x * WG;
+    const uint32_t sb = smem_u32(sB);
+
+    uint64_t rb = (uint64_t)blockIdx.x * WG + wg;
+    AFeat next = load_afeat(P.fobj, P.n, rb * kRows + r_in, q);
+    for (; rb < n_rb; rb += rb_step) {
+        const AFeat cur = next;
+        next = load_afeat(P.fobj, P.n, (rb + rb_step) * kRows + r_in, q);
+        uint32_t a[3][4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            __nv_bfloat16 h0, m0, l0, h1, m1, l1;
+            split3(cur.v[i].x, h0, m0, l0);
+            split3(cur.v[i].y, h1, m1, l1);
+            a[0][i] = pack2(h0, h1); a[1][i] = pack2(m0, m1); a[2][i] = pack2(l0, l1);
+        }
+        float lv[2][RT];
+        uint32_t lp[2][RT], ld[2][RT];
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int i = 0; i < RT; i++) { lv[h][i] = -INFINITY; lp[h][i] = kNone; ld[h][i] = kNone; }
+        float acc[NT / 2];
+        for (uint32_t t = 0; t < n_tiles; t++) {
+            issue_tile<NT>(acc, a, sb, b_block_bytes, t, P.m_pad);
+            wgmma_wait<0>();
+            fence_regs(acc);
+            const uint32_t col_base = t * NT;
+            if (col_base + NT > P.n_live) {   // warp-uniform: only the padded tail of the last tile
+#pragma unroll
+                for (int i = 0; i < NT / 2; i++)
+                    if (col_base + 8 * (i >> 2) + 2 * q + (i & 1) >= P.n_live) acc[i] = -INFINITY;
+            }
+#pragma unroll
+            for (int i = 0; i < NT / 2; i++) {   // increasing column within each row h = (i >> 1) & 1
+                const int h = (i >> 1) & 1;
+                const uint32_t col = col_base + 8 * (i >> 2) + 2 * q + (i & 1);
+                if (acc[i] > lv[h][RT - 1]) insert_dom<RT>(lv[h], lp[h], ld[h], acc[i], col, __ldg(pdom + col));
+            }
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+#pragma unroll
+            for (int d = 1; d <= 2; d <<= 1) {
+                float ov[RT];
+                uint32_t op[RT], od[RT];
+#pragma unroll
+                for (int i = 0; i < RT; i++) {
+                    ov[i] = __shfl_xor_sync(0xFFFFFFFFu, lv[h][i], d);
+                    op[i] = __shfl_xor_sync(0xFFFFFFFFu, lp[h][i], d);
+                    od[i] = __shfl_xor_sync(0xFFFFFFFFu, ld[h][i], d);
+                }
+#pragma unroll
+                for (int i = 0; i < RT; i++)
+                    if (col_before(ov[i], op[i], lv[h][RT - 1], lp[h][RT - 1])) insert_dom<RT>(lv[h], lp[h], ld[h], ov[i], op[i], od[i]);
+            }
+            const uint64_t row = rb * kRows + r_in + 8 * h;
+            if (q == 0 && row < P.n) {
+#pragma unroll
+                for (int i = 0; i < RT; i++) P.out_idx[row * RT + i] = lp[h][i];
+            }
+        }
+    }
+}
+
+// Second pass of the failure-domain lists: eight lanes per object, as in k_affinity_resolve_ranked.  Lane r re-costs column r of the
+// first entry's group and candidate r, both with k_affinity_resolve's fmaf order.  Rank 1 is the smallest (cost, position) of that
+// group, exactly as k_affinity_resolve picks it; ranks 2.. are the smallest remaining (cost, position) among the candidates whose
+// domain is not listed yet, and each pick masks every candidate of its domain (rank 1's included).
+template <int RT>
+__global__ void __launch_bounds__(256, 2)
+k_affinity_resolve_spread(const float *__restrict__ fobj, uint64_t n, const float *__restrict__ fnode_g, const uint32_t *__restrict__ nidx_map,
+                          const uint32_t *__restrict__ pdom, uint32_t n_live, const uint32_t *__restrict__ cols, uint32_t ranks, uint32_t *__restrict__ out) {
+    const uint32_t lane = threadIdx.x & 31, r = lane & 7, seg = lane & ~7u;
+    const uint32_t q = lane >> 3;
+    const uint64_t warp0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    const float4 *fobj4 = reinterpret_cast<const float4 *>(fobj);
+    const float4 *fnode4 = reinterpret_cast<const float4 *>(fnode_g);   // piece k of position p: + ((p >> 3) * 4 + k) * 8 + (p & 7)
+    auto cost_key = [&](const float4 (&o)[4], uint32_t p) {
+        const float4 *fn = fnode4 + (size_t)(p >> 3) * 32 + (p & 7);
+        float a = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            const float4 x = __ldg(fn + k * 8);
+            a = fmaf(o[k].x, x.x, a); a = fmaf(o[k].y, x.y, a); a = fmaf(o[k].z, x.z, a); a = fmaf(o[k].w, x.w, a);
+        }
+        const uint32_t bits = __float_as_uint(-a);
+        return (int)(bits ^ ((uint32_t)((int)bits >> 31) & 0x7FFFFFFFu));
+    };
+    // smallest (key, position) over the 8 lanes of an object, its domain carried along
+    auto seg_min = [](int &k, uint32_t &p, uint32_t &dm) {
+#pragma unroll
+        for (int d = 4; d >= 1; d >>= 1) {
+            const int ok = __shfl_xor_sync(0xFFFFFFFFu, k, d);
+            const uint32_t op = __shfl_xor_sync(0xFFFFFFFFu, p, d), od = __shfl_xor_sync(0xFFFFFFFFu, dm, d);
+            if (ok < k || (ok == k && op < p)) { k = ok; p = op; dm = od; }
+        }
+    };
+    // one trip ahead, as in k_affinity_resolve: the candidates and the row of the next trip are in flight while this trip scores
+    uint64_t base = warp0 * 4;
+    bool mine = base + q < n;
+    uint64_t row = mine ? base + q : n - 1;
+    uint32_t c = kNone;
+    float4 o[4] = {};
+    if (base < n) {
+        if (r < RT) c = __ldg(cols + row * RT + r);
+#pragma unroll
+        for (int k = 0; k < 4; k++) o[k] = __ldg(fobj4 + row * 4 + k);
+    }
+    for (; base < n; base += nwarps * 4) {
+        const uint64_t nbase = base + nwarps * 4;
+        const bool nmine = nbase + q < n;
+        const uint64_t nrow = nmine ? nbase + q : n - 1;
+        uint32_t nc = kNone;
+        float4 no[4] = {};
+        if (nbase < n) {
+            if (r < RT) nc = __ldg(cols + nrow * RT + r);
+#pragma unroll
+            for (int k = 0; k < 4; k++) no[k] = __ldg(fobj4 + nrow * 4 + k);
+        }
+        // rank 1: column r of the first entry's group (group 0 when no column was listed, as k_affinity_wgmma's initial group)
+        const uint32_t c0 = __shfl_sync(0xFFFFFFFFu, c, seg);
+        uint32_t p1 = (c0 == kNone ? 0u : c0 >> 3) * 8 + r;
+        int k1 = cost_key(o, p1);
+        if (p1 >= n_live) { k1 = 0x7F800000; p1 = kNone; }
+        uint32_t d1 = 0;
+        seg_min(k1, p1, d1);
+        d1 = __ldg(pdom + p1);   // p1 < n_live: the group holds the listed column, or is group 0
+        // candidate r: its domain masked out once listed
+        int kc = 0x7F800000;
+        uint32_t pc = kNone, dc = kNone;
+        if (c != kNone) { kc = cost_key(o, c); pc = c; dc = __ldg(pdom + c); }
+        if (r == 0 && mine) out[row * ranks] = __ldg(nidx_map + p1);
+        uint32_t dl = d1;
+        for (uint32_t rank = 1; rank < ranks; rank++) {   // warp-uniform
+            if (dc == dl) { kc = 0x7F800000; pc = kNone; dc = kNone; }
+            int k = kc;
+            uint32_t p = pc, dm = dc;
+            seg_min(k, p, dm);
+            if (r == 0 && mine) out[row * ranks + rank] = p == kNone ? kNone : __ldg(nidx_map + p);
+            dl = dm;   // kNone once nothing is left: it masks only empty slots
+        }
+        mine = nmine; row = nrow; c = nc;
+#pragma unroll
+        for (int k = 0; k < 4; k++) o[k] = no[k];
+    }
+}
+
 }  // namespace
 
 // development hook: device buffer of 16 u64 per CTA that receives the tensor-core kernel's setup and total cycle counts
@@ -608,6 +806,54 @@ cudaError_t launch_assign_affinity_umma_ranked(const Launch &L, const float *d_f
         case 2: return launch_ranked_pair<2>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
         case 4: return launch_ranked_pair<4>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
         default: return launch_ranked_pair<8>(L, P, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+    }
+}
+
+namespace {
+
+// warpgroups per CTA of k_affinity_wgmma_spread<NT, RT>: the lists cost 6 RT registers per thread; four warpgroups where they fit in
+// 128 registers without spills (ptxas -v)
+constexpr int spread_warpgroups(int RT) { return RT <= 4 ? 4 : 2; }
+
+template <int NT, int RT>
+cudaError_t launch_wgmma_spread(const Launch &L, const WgmmaParams &P, const uint32_t *d_pdom, size_t smem) {
+    constexpr int WG = spread_warpgroups(RT);
+    const uint64_t n_rb = (P.n + kRows - 1) / kRows, n_cta = (n_rb + WG - 1) / WG;
+    const int grid = (int)(n_cta < (uint64_t)L.sm_count ? n_cta : (uint64_t)L.sm_count);
+    cudaError_t err = cudaFuncSetAttribute(k_affinity_wgmma_spread<NT, RT, WG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (err == cudaSuccess) k_affinity_wgmma_spread<NT, RT, WG><<<grid, 128 * WG, smem, L.stream>>>(P, d_pdom);
+    return err == cudaSuccess ? cudaGetLastError() : err;
+}
+
+template <int RT>
+cudaError_t launch_spread_pair(const Launch &L, const WgmmaParams &P, const uint32_t *d_pdom, size_t smem, const float *d_fnode_g, const uint32_t *d_nidx_map,
+                               uint32_t ranks, uint32_t *d_out_idx) {
+    const cudaError_t err = P.m_pad <= 64 ? launch_wgmma_spread<64, RT>(L, P, d_pdom, smem) : launch_wgmma_spread<128, RT>(L, P, d_pdom, smem);
+    if (err != cudaSuccess) return err;
+    RIO_COUNT_LAUNCH(L);
+    const uint64_t blocks = (P.n + 31) / 32, cap = (uint64_t)L.sm_count * 8;
+    k_affinity_resolve_spread<RT><<<(int)(blocks < cap ? blocks : cap), 256, 0, L.stream>>>(P.fobj, P.n, d_fnode_g, d_nidx_map, d_pdom, P.n_live, P.out_idx,
+                                                                                           ranks, d_out_idx);
+    RIO_COUNT_LAUNCH(L);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+cudaError_t launch_assign_affinity_umma_spread(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode_c, const float *d_fnode_g,
+                                               const uint32_t *d_nidx_map, const uint32_t *d_pdom, uint32_t n_live, uint32_t m_pad, uint32_t ranks,
+                                               uint32_t *d_cols, uint32_t *d_out_idx) {
+    if (!n) return cudaSuccess;
+    const bool small = m_pad <= 64;
+    if (!n_live || (small && m_pad != 64) || (!small && (m_pad % 256)) || m_pad > affinity_umma_max_nodes() || ranks < 1 || ranks > kMaxRanks)
+        return cudaErrorInvalidValue;
+    const size_t smem = (size_t)3 * m_pad * 32;
+    const WgmmaParams P{d_fobj, n, d_fnode_c, n_live, m_pad, d_cols, nullptr};
+    switch (affinity_ranked_groups(ranks)) {
+        case 1: return launch_spread_pair<1>(L, P, d_pdom, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        case 2: return launch_spread_pair<2>(L, P, d_pdom, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        case 4: return launch_spread_pair<4>(L, P, d_pdom, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
+        default: return launch_spread_pair<8>(L, P, d_pdom, smem, d_fnode_g, d_nidx_map, ranks, d_out_idx);
     }
 }
 

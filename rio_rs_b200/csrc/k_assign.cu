@@ -7,6 +7,7 @@
 // The kernel is integer-ALU bound (12 B of HBM traffic per object against M pair hashes), see DESIGN.md 5.1.
 #include "kernels.cuh"
 #include "k_affinity_ranked.cuh"
+#include "k_affinity_spread.cuh"
 #include "spec.cuh"
 #include <cstdlib>
 
@@ -413,10 +414,13 @@ k_assign_affinity_generic(const float *__restrict__ fobj, uint64_t n, const floa
 // one object per thread, and the RT smallest (cost, j) kept sorted in registers.  A node displaces an entry only with a strictly
 // smaller cost, so equal costs keep the lower j first and the first entry is the unranked kernels' node.  KC = 16 keeps the object
 // row in registers; KC = 0 takes any K at run time.  The first `ranks` (<= RT) entries are written, kNone past the live set.
-template <int KC, int RT>
+// SPREAD (DESIGN.md 3.14): the list keeps one entry per failure domain (ndom: dense domain id per interned index).  A node of a
+// listed domain replaces that entry only with a strictly smaller cost; any other node enters only by beating the last entry.  The
+// list is then the best RT domain representatives, so its first `ranks` entries are the failure-domain list.
+template <int KC, int RT, bool SPREAD>
 __global__ void __launch_bounds__(kAssignThreads)
 k_assign_affinity_ranked(const float *__restrict__ fobj, uint64_t n, const float *__restrict__ fnode, const uint32_t *__restrict__ live,
-                         uint32_t n_total, uint32_t K, uint32_t ranks, uint32_t *__restrict__ out_idx) {
+                         uint32_t n_total, uint32_t K, uint32_t ranks, uint32_t *__restrict__ out_idx, const uint32_t *__restrict__ ndom) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
         float fo[KC ? KC : 1];
         if constexpr (KC != 0) {
@@ -428,9 +432,13 @@ k_assign_affinity_ranked(const float *__restrict__ fobj, uint64_t n, const float
             }
         }
         float lc[RT];
-        uint32_t lj[RT];
+        uint32_t lj[RT], ld[SPREAD ? RT : 1];
 #pragma unroll
         for (int s = 0; s < RT; s++) { lc[s] = 0.f; lj[s] = kNone; }
+        if constexpr (SPREAD) {
+#pragma unroll
+            for (int s = 0; s < RT; s++) ld[s] = kNone;
+        }
         for (uint32_t j = 0; j < n_total; j++) {
             if (!__ldg(live + j)) continue;
             float acc = 0.f;
@@ -450,12 +458,34 @@ k_assign_affinity_ranked(const float *__restrict__ fobj, uint64_t n, const float
             }
             const float cst = -acc;
             if (lj[RT - 1] != kNone && !(cst < lc[RT - 1])) continue;
+            if constexpr (SPREAD) {
+                // j is larger than every listed index, so "listed before it" is "cost not larger"; the swap chain below carries
+                // listed entries, which compare by (cost, index), and stops at the entry of the candidate's own domain
+                const uint32_t dc = __ldg(ndom + j);
+                bool keep = true;
 #pragma unroll
-            for (int s = RT - 1; s > 0; s--) {
-                if (lj[s - 1] == kNone || cst < lc[s - 1]) { lc[s] = lc[s - 1]; lj[s] = lj[s - 1]; }
-                else if (lj[s] == kNone || cst < lc[s]) { lc[s] = cst; lj[s] = j; }
+                for (int s = 0; s < RT; s++) keep &= !(ld[s] == dc && !(cst < lc[s]));
+                if (!keep) continue;
+                float c = cst;
+                uint32_t cj = j, cd = dc;
+                bool go = true;
+#pragma unroll
+                for (int s = 0; s < RT; s++) {
+                    const bool sw = go && (lj[s] == kNone || c < lc[s] || (c == lc[s] && cj < lj[s]));
+                    const float tc = lc[s];
+                    const uint32_t tj = lj[s], td = ld[s];
+                    lc[s] = sw ? c : tc; lj[s] = sw ? cj : tj; ld[s] = sw ? cd : td;
+                    c = sw ? tc : c; cj = sw ? tj : cj; cd = sw ? td : cd;
+                    go = go && !(sw && td == dc);
+                }
+            } else {
+#pragma unroll
+                for (int s = RT - 1; s > 0; s--) {
+                    if (lj[s - 1] == kNone || cst < lc[s - 1]) { lc[s] = lc[s - 1]; lj[s] = lj[s - 1]; }
+                    else if (lj[s] == kNone || cst < lc[s]) { lc[s] = cst; lj[s] = j; }
+                }
+                if (lj[0] == kNone || cst < lc[0]) { lc[0] = cst; lj[0] = j; }
             }
-            if (lj[0] == kNone || cst < lc[0]) { lc[0] = cst; lj[0] = j; }
         }
 #pragma unroll
         for (int s = 0; s < RT; s++)
@@ -643,23 +673,31 @@ void launch_assign_affinity(const Launch &L, const float *d_fobj, uint64_t n, co
     RIO_COUNT_LAUNCH(L);
 }
 
-template <int KC>
+template <int KC, bool SPREAD>
 static void launch_affinity_ranked_k(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode, const uint32_t *d_live, uint32_t n_total,
-                                     uint32_t K, uint32_t ranks, uint32_t *d_out_idx) {
+                                     uint32_t K, uint32_t ranks, uint32_t *d_out_idx, const uint32_t *d_ndom) {
     const int grid = grid_for(n, kAssignThreads, L.sm_count, 8);
     switch (affinity_ranked_groups(ranks)) {
-        case 1: k_assign_affinity_ranked<KC, 1><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
-        case 2: k_assign_affinity_ranked<KC, 2><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
-        case 4: k_assign_affinity_ranked<KC, 4><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
-        default: k_assign_affinity_ranked<KC, 8><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx); break;
+        case 1: k_assign_affinity_ranked<KC, 1, SPREAD><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom); break;
+        case 2: k_assign_affinity_ranked<KC, 2, SPREAD><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom); break;
+        case 4: k_assign_affinity_ranked<KC, 4, SPREAD><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom); break;
+        default: k_assign_affinity_ranked<KC, 8, SPREAD><<<grid, kAssignThreads, 0, L.stream>>>(d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom); break;
     }
 }
 
 void launch_assign_affinity_ranked(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode, const uint32_t *d_live, uint32_t n_total,
                                    uint32_t K, uint32_t ranks, uint32_t *d_out_idx) {
     if (!n) return;
-    if (K == 16) launch_affinity_ranked_k<16>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx);
-    else launch_affinity_ranked_k<0>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx);
+    if (K == 16) launch_affinity_ranked_k<16, false>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, nullptr);
+    else launch_affinity_ranked_k<0, false>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, nullptr);
+    RIO_COUNT_LAUNCH(L);
+}
+
+void launch_assign_affinity_spread(const Launch &L, const float *d_fobj, uint64_t n, const float *d_fnode, const uint32_t *d_live, uint32_t n_total,
+                                   uint32_t K, const uint32_t *d_ndom, uint32_t ranks, uint32_t *d_out_idx) {
+    if (!n) return;
+    if (K == 16) launch_affinity_ranked_k<16, true>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom);
+    else launch_affinity_ranked_k<0, true>(L, d_fobj, n, d_fnode, d_live, n_total, K, ranks, d_out_idx, d_ndom);
     RIO_COUNT_LAUNCH(L);
 }
 

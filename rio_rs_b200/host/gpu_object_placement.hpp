@@ -141,6 +141,14 @@ class GpuObjectPlacement {
         check(rio_cuda_assign_ranked_affinity_batch(e_->h, obj_feats.data(), n, ranks, out.data()));
         return out;
     }
+    // each object's `ranks` lowest-cost live nodes in distinct failure domains under the affinity cost (DESIGN.md 3.14), arguments
+    // and result as for assign_ranked_affinity
+    std::vector<uint32_t> assign_ranked_affinity_spread(const std::vector<float> &obj_feats, size_t n, uint32_t ranks) const {
+        if (n && obj_feats.size() % n) throw ObjectPlacementError(ObjectPlacementError::Unknown, "obj_feats is not n x K");
+        std::vector<uint32_t> out(n * ranks);
+        check(rio_cuda_assign_ranked_affinity_spread_batch(e_->h, obj_feats.data(), n, ranks, out.data()));
+        return out;
+    }
     std::vector<uint32_t> place_batch(const std::vector<uint64_t> &keys, uint32_t policy, uint32_t self_idx) const {
         std::vector<uint32_t> out(keys.size());
         check(rio_cuda_place_batch(e_->h, keys.data(), keys.size(), policy, self_idx, out.data()));

@@ -316,6 +316,16 @@ class GpuObjectPlacement:
         self._ck(self.L.rio_cuda_assign_ranked_affinity_batch(self.h, _ptr(obj_feats), n, ranks, _ptr(out)))
         return out
 
+    def assign_ranked_affinity_spread(self, obj_feats, ranks):
+        """Each object's `ranks` lowest-cost live nodes in distinct failure domains under the affinity cost (DESIGN.md 3.14) ->
+        (n, ranks) uint32: column 0 is assign_batch(obj_feats=...), column 1 where the object goes when column 0's whole domain
+        leaves; RIO_NONE past the live domain count."""
+        obj_feats = np.ascontiguousarray(obj_feats, dtype=np.float32)
+        n = obj_feats.shape[0]
+        out = np.empty((n, ranks), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_assign_ranked_affinity_spread_batch(self.h, _ptr(obj_feats), n, ranks, _ptr(out)))
+        return out
+
     def assign_bounded_batch(self, keys, n_total=0, cap_num=5, cap_den=4, max_rounds=4, out=None):
         """assign_batch + bounded-load rounds for host buffers; returns (indices, passes)."""
         keys = np.ascontiguousarray(keys, dtype=np.uint64)

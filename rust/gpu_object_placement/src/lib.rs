@@ -179,6 +179,17 @@ impl GpuObjectPlacement {
         check(self.h(), unsafe { sys::rio_cuda_assign_ranked_affinity_batch(self.h(), obj_feats.as_ptr(), n, ranks, out.as_mut_ptr()) })?;
         Ok(out)
     }
+    /// Each object's `ranks` lowest-cost live nodes in distinct failure domains under the affinity cost (DESIGN.md 3.14).  Arguments
+    /// and result as for `assign_ranked_affinity`; rank 2 is where the object goes when rank 1's whole domain leaves.
+    pub fn assign_ranked_affinity_spread(&self, obj_feats: &[f32], n: usize, ranks: u32) -> Result<Vec<u32>, ObjectPlacementError> {
+        if n != 0 && obj_feats.len() % n != 0 {
+            return Err(ObjectPlacementError::Unknown("obj_feats is not n x K".into()));
+        }
+        let len = n.checked_mul(ranks as usize).ok_or_else(|| ObjectPlacementError::Unknown("n x ranks overflows".into()))?;
+        let mut out = vec![sys::RIO_NONE; len];
+        check(self.h(), unsafe { sys::rio_cuda_assign_ranked_affinity_spread_batch(self.h(), obj_feats.as_ptr(), n, ranks, out.as_mut_ptr()) })?;
+        Ok(out)
+    }
     /// Eager re-placement after a membership event (beside peer_to_peer.rs:170-191).
     pub fn rebalance(&self, join: bool, node_idx: u32) -> Result<u64, ObjectPlacementError> {
         let mut moved = 0u64;

@@ -79,6 +79,7 @@ extern "C" {
     pub fn rio_cuda_assign_ranked_batch(h: *mut rio_placement, keys: *const u64, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_spread_batch(h: *mut rio_placement, keys: *const u64, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_affinity_batch(h: *mut rio_placement, obj_feats: *const f32, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_affinity_spread_batch(h: *mut rio_placement, obj_feats: *const f32, n: size_t, ranks: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_place_batch(h: *mut rio_placement, keys: *const u64, n: size_t, policy: u32, self_idx: u32, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_rebalance(h: *mut rio_placement, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_rebalance_changes(h: *mut rio_placement, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
@@ -121,6 +122,7 @@ extern "C" {
     pub fn rio_cuda_assign_ranked_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_spread_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_ranked_affinity_batch_dev(h: *mut rio_placement, d_obj_feats: *const f32, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_ranked_affinity_spread_batch_dev(h: *mut rio_placement, d_obj_feats: *const f32, n: size_t, ranks: u32, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_lookup_batch_dev(h: *mut rio_placement, d_keys: *const u64, n: size_t, d_out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_upsert_batch_dev(h: *mut rio_placement, d_keys: *const u64, d_idx: *const u32, n: size_t) -> rio_status;
 
