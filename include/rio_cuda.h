@@ -252,7 +252,7 @@ rio_status  rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, c
  * receives the number of objects whose rank 1 changed, out_changed (may be NULL) the number whose list changed at any rank.
  * RIO_ERR_UNKNOWN: ranks outside [1, RIO_MAX_RANKS], n x ranks overflowing, a read outside the set, NULL buffers, the argument
  * errors of rio_cuda_set_rebalance_changes, a set holding no lists, or a change set under another solver or trie_bits than the
- * lists were computed with.  RIO_ERR_UPSTREAM when the library was built without the ranked-set kernels.  Every call that rewrites
+ * lists were computed with (affinity lists ignore the solver: see rio_cuda_set_assign_ranked_affinity below).  RIO_ERR_UPSTREAM when the library was built without the ranked-set kernels.  Every call that rewrites
  * the set's assignment otherwise (set_load_keys, set_synth_keys, set_assign, set_assign_bounded(_begin), set_rebalance,
  * set_rebalance_changes) drops the lists. */
 rio_status  rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks);
@@ -268,6 +268,29 @@ rio_status  rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t 
  * when the library was built without the spread-set kernels.  The calls that drop ranked lists drop these too, and
  * rio_cuda_set_assign_ranked makes the set a plain ranked set again (plain ranked sets ignore labels). */
 rio_status  rio_cuda_set_assign_ranked_spread(rio_objset *s, uint32_t ranks);
+/* Affinity resident sets (DESIGN.md 3.15).  rio_cuda_set_assign_ranked_affinity(_spread) works as rio_cuda_set_assign_ranked, with
+ * each object's list from rio_cuda_assign_ranked_affinity_batch (or rio_cuda_assign_ranked_affinity_spread_batch) of the set's
+ * features (rio_cuda_set_load_feats) in place of its ranked list, on the path that call takes now (column 0 is then bit for bit rio_cuda_set_assign(use_affinity = 1) on that path).  The
+ * set records the kind of lists, the path (tensor cores or CUDA cores; RIO_AFFINITY_VARIANT is read here only), the handle's K, every
+ * interned node's feature row and, for failure-domain lists, its label.  rio_cuda_set_read_ranked reads these lists unchanged.
+ * On such a set rio_cuda_set_rebalance_changes_ranked ignores the solver and trie_bits and classifies by liveness (active, weight > 0):
+ *   REPLACE    = every interned node not live now, every live node whose feature row differs from the recorded one (refeatured) and,
+ *                for failure-domain lists, every relabelled live node;
+ *   CANDIDATES = every changed node live now with prev_weight 0, and every refeatured or relabelled live node;
+ *   a live -> live weight change is a no-op.
+ * A list with a member in REPLACE, or with no member, is recomputed on the recorded path; any other becomes the first `ranks` of
+ * itself u CANDIDATES in (fp32 cost, node index) order (for failure-domain lists the best `ranks` domain representatives).  k = 0
+ * with a refeature or relabel applies it, k = 0 without one does nothing.  On the CUDA cores the lists then equal a fresh CUDA-core
+ * call over the current live set, features and labels bit for bit.  On the tensor cores they agree with a fresh call but for near-ties
+ * within the tolerance of 3.9, and column 0 of a row a candidate entered can differ from rio_cuda_set_assign(use_affinity = 1) at a
+ * near-tie.  A tensor-core set recomputes on the CUDA cores while its padded live count exceeds the tensor path's limit.
+ * RIO_ERR_UNKNOWN: ranks outside [1, RIO_MAX_RANKS], n x ranks overflowing, a handle without node features, set features missing or
+ * of another K than the handle's, and on a change set the argument errors of rio_cuda_set_rebalance_changes or a handle K other than
+ * the recorded one (a refused call leaves lists and records as they were).  RIO_ERR_UPSTREAM when the library was built without the
+ * affinity-set kernels.  Every call that drops ranked lists drops these, and so does rio_cuda_set_load_feats;
+ * rio_cuda_set_assign_ranked(_spread) makes the set a hash-policy set again. */
+rio_status  rio_cuda_set_assign_ranked_affinity(rio_objset *s, uint32_t ranks);
+rio_status  rio_cuda_set_assign_ranked_affinity_spread(rio_objset *s, uint32_t ranks);
 /* Global (all ranks) per-node counters of the set's current assignment. */
 rio_status  rio_cuda_set_counters(rio_objset *s, uint32_t *out, uint32_t cap);
 rio_status  rio_cuda_set_read(rio_objset *s, uint64_t first, uint64_t n, uint64_t *out_keys, uint32_t *out_idx);

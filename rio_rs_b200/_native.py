@@ -89,6 +89,8 @@ SIGNATURES = {
     "rio_cuda_set_read_ranked": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp]),
     "rio_cuda_set_rebalance_changes_ranked": (C.c_int32, [H, vp, vp, sz, u64p, u64p]),
     "rio_cuda_set_assign_ranked_spread": (C.c_int32, [H, C.c_uint32]),
+    "rio_cuda_set_assign_ranked_affinity": (C.c_int32, [H, C.c_uint32]),
+    "rio_cuda_set_assign_ranked_affinity_spread": (C.c_int32, [H, C.c_uint32]),
     "rio_cuda_set_counters": (C.c_int32, [H, vp, C.c_uint32]),
     "rio_cuda_set_read": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp, vp]),
     "rio_cuda_set_size": (C.c_int32, [H, u64p]),

@@ -10,6 +10,7 @@
 #include "k_ranked.cuh"
 #include "k_affinity_ranked.cuh"
 #include "k_affinity_spread.cuh"
+#include "k_affinity_set.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -205,6 +206,9 @@ struct rio_placement {
     DevBuf aff_dom;
     size_t aff_dom_pos = 0;                        // offset of the per-position ids in aff_dom
     uint64_t aff_dom_version[2] = {~0ull, ~0ull};
+    // bumped by every call that sets node features (set_nodes with feats, node_upsert with feat): the affinity resident sets compare
+    // their feature snapshot only when it moved (DESIGN.md 3.15)
+    uint64_t feat_version = 0;
     unsigned long long *d_scalars = nullptr;   // S_COUNT u64 + error u32
     unsigned long long *h_scalars = nullptr;   // pinned mirror
 
@@ -244,7 +248,14 @@ struct rio_objset {
     bool spread = false;
     std::vector<uint32_t> label_snap;
     uint64_t label_snap_version = 0;
-    void drop_lists() { ranks = 0; spread = false; }
+    // affinity lists (DESIGN.md 3.15): the lists are affinity lists of the set's features (spread says which kind), computed on the
+    // tensor cores (aff_tensor) or the CUDA cores under the handle's K aff_K, with the node features of feat_snap (aff_K floats per node
+    // interned then; a row that was not K wide is zeros, as the kernels see it), the handle's at feat_version feat_snap_version
+    bool affinity = false, aff_tensor = false;
+    uint32_t aff_K = 0;
+    std::vector<float> feat_snap;
+    uint64_t feat_snap_version = 0;
+    void drop_lists() { ranks = 0; spread = false; affinity = false; }
 };
 
 namespace {
@@ -661,9 +672,12 @@ void run_assign_spread(rio_placement *h, const uint64_t *d_keys, uint64_t n, uin
 // affinity dispatch: no live node fills the output with NONE; the tensor-core (wgmma) kernel for K == 16 (unless
 // RIO_AFFINITY_VARIANT=ffma or the node set does not fit); else the CUDA cores
 enum class AffinityPath { kNoLiveNode, kTensorCores, kCudaCores };
-AffinityPath affinity_path(const rio_placement *h) {
+bool affinity_umma_wanted() {
     const char *v = getenv("RIO_AFFINITY_VARIANT");
-    const bool want_umma = !(v && v[0] == 'f');
+    return !(v && v[0] == 'f');
+}
+// want_umma = false keeps K == 16 on the CUDA cores (an affinity resident set recorded there, DESIGN.md 3.15)
+AffinityPath affinity_path(const rio_placement *h, bool want_umma = affinity_umma_wanted()) {
     if (!h->aff_live && h->K == 16 && h->tabs.tab.n_live == 0) return AffinityPath::kNoLiveNode;
     if (want_umma && h->K == 16 && h->aff_live && h->aff_pad <= affinity_umma_max_nodes()) return AffinityPath::kTensorCores;
     return AffinityPath::kCudaCores;
@@ -684,11 +698,11 @@ void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d
 }
 
 // each object's `ranks` lowest-cost live nodes (DESIGN.md 3.9), on the path run_affinity takes for the same handle and environment,
-// so that rank 1 is its answer; the tensor-core pair keeps its per-object groups in s_idx2 between the two passes
-void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+// so that rank 1 is its answer, or on `path`; the tensor-core pair keeps its per-object groups in s_idx2 between the two passes
+void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx, AffinityPath path) {
     if (!launch_assign_affinity_ranked || !launch_assign_affinity_umma_ranked)
         throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked affinity kernels (k_affinity_umma.cu / k_assign.cu are not linked)"};
-    switch (affinity_path(h)) {
+    switch (path) {
         case AffinityPath::kNoLiveNode: launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); break;
         case AffinityPath::kTensorCores:
             h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
@@ -724,11 +738,10 @@ void ensure_aff_dom(rio_placement *h) {
 }
 
 // each object's `ranks` lowest-cost live nodes in distinct failure domains (DESIGN.md 3.14), on the path run_affinity takes, so that
-// rank 1 is its answer; the tensor-core pair keeps each object's listed column positions in s_idx2 between the two passes
-void run_affinity_spread(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
+// rank 1 is its answer, or on `path`; the tensor-core pair keeps each object's listed column positions in s_idx2 between the two passes
+void run_affinity_spread(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx, AffinityPath path) {
     if (!launch_assign_affinity_spread || !launch_assign_affinity_umma_spread)
         throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no failure-domain affinity kernels (k_affinity_spread.cuh launchers are not linked)"};
-    const AffinityPath path = affinity_path(h);
     if (path == AffinityPath::kNoLiveNode) { launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); return; }
     ensure_aff_dom(h);
     const uint32_t *ndom = h->aff_dom.as<uint32_t>();
@@ -1180,7 +1193,7 @@ rio_status rio_cuda_set_nodes(rio_placement *h, const char *const *addrs, const 
     return guarded(h, [&] {
         REQUIRE(M == 0 || addrs, "addrs is NULL");
         REQUIRE(!feats || K > 0, "feats given with K == 0");
-        if (feats) { h->K = K; for (auto &ni : h->nodes) ni.feat.clear(); }
+        if (feats) { h->K = K; for (auto &ni : h->nodes) ni.feat.clear(); h->feat_version++; }
         for (auto &ni : h->nodes) ni.active = false;
         for (uint32_t j = 0; j < M; j++) {
             REQUIRE(addrs[j], "null address");
@@ -1203,7 +1216,7 @@ rio_status rio_cuda_node_upsert(rio_placement *h, const char *address, uint32_t 
         NodeInfo &ni = h->nodes[idx];
         ni.weight = weight;
         ni.active = true;
-        if (feat) { REQUIRE(K > 0 && (h->K == 0 || h->K == K), "feature dimension mismatch"); h->K = K; ni.feat.assign(feat, feat + K); }
+        if (feat) { REQUIRE(K > 0 && (h->K == 0 || h->K == K), "feature dimension mismatch"); h->K = K; ni.feat.assign(feat, feat + K); h->feat_version++; }
         h->tab_dirty = true;
         if (out_idx) *out_idx = idx;
     });
@@ -1496,7 +1509,7 @@ rio_status rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *
         REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
         ensure_tab(h);
         ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
-                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_ranked(h, d_feats, n, ranks, d_out); });
+                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_ranked(h, d_feats, n, ranks, d_out, affinity_path(h)); });
     });
 }
 
@@ -1508,7 +1521,7 @@ rio_status rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const flo
         REQUIRE(d_obj_feats && d_out_idx, "null buffer");
         REQUIRE(h->K > 0, "assign with object features needs node features");
         ensure_tab(h);
-        run_affinity_ranked(h, d_obj_feats, n, ranks, d_out_idx);
+        run_affinity_ranked(h, d_obj_feats, n, ranks, d_out_idx, affinity_path(h));
     });
 }
 
@@ -1522,7 +1535,7 @@ rio_status rio_cuda_assign_ranked_affinity_spread_batch(rio_placement *h, const 
         REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
         ensure_tab(h);
         ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
-                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_spread(h, d_feats, n, ranks, d_out); });
+                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_spread(h, d_feats, n, ranks, d_out, affinity_path(h)); });
     });
 }
 
@@ -1534,7 +1547,7 @@ rio_status rio_cuda_assign_ranked_affinity_spread_batch_dev(rio_placement *h, co
         REQUIRE(d_obj_feats && d_out_idx, "null buffer");
         REQUIRE(h->K > 0, "assign with object features needs node features");
         ensure_tab(h);
-        run_affinity_spread(h, d_obj_feats, n, ranks, d_out_idx);
+        run_affinity_spread(h, d_obj_feats, n, ranks, d_out_idx, affinity_path(h));
     });
 }
 
@@ -1837,6 +1850,7 @@ rio_status rio_cuda_set_load_feats(rio_objset *s, const float *feats, uint32_t K
         s->feats.ensure(s->n * (size_t)K * 4, h->stream);
         CUDA_TRY(cudaMemcpyAsync(s->feats.p, feats, s->n * (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
         s->K = K;
+        if (s->affinity) s->drop_lists();   // affinity lists are lists of the features just replaced; hash lists stay
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
@@ -2032,6 +2046,136 @@ void set_assign_lists(rio_objset *s, uint32_t ranks, bool spread) {
     if (spread) snapshot_labels(s);
 }
 
+// ---- affinity resident sets (DESIGN.md 3.15) ------------------------------------------------------------------------------------
+void require_affinity_set_kernels(bool spread) {
+    const bool have = launch_ranked_primary && launch_scatter_ranked && launch_rebalance_changes_affinity && launch_gather_rows &&
+                      (spread ? launch_assign_affinity_spread && launch_assign_affinity_umma_spread
+                              : launch_assign_affinity_ranked && launch_assign_affinity_umma_ranked);
+    if (!have) throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no affinity-set kernels (k_affinity_set.cuh launchers are not linked)"};
+}
+
+// the handle's node features, as the kernels see them (K floats per interned node, zeros for a row that is not K wide), become the
+// set's snapshot
+void snapshot_feats(rio_objset *s) {
+    const rio_placement *h = s->h;
+    const uint32_t K = h->K;
+    s->feat_snap.assign(h->nodes.size() * K, 0.f);
+    for (size_t j = 0; j < h->nodes.size(); j++)
+        if (h->nodes[j].feat.size() == K) std::copy(h->nodes[j].feat.begin(), h->nodes[j].feat.end(), s->feat_snap.begin() + j * K);
+    s->feat_snap_version = h->feat_version;
+}
+
+// live nodes whose feature row differs bitwise from the set's snapshot; a node interned after the snapshot counts as refeatured
+std::vector<uint32_t> refeatured_live(const rio_objset *s) {
+    const rio_placement *h = s->h;
+    std::vector<uint32_t> out;
+    if (s->feat_snap_version == h->feat_version) return out;
+    const uint32_t K = s->aff_K;
+    const size_t snap_n = s->feat_snap.size() / K;
+    const std::vector<float> zeros(K, 0.f);
+    for (uint32_t j = 0; j < (uint32_t)h->nodes.size(); j++) {
+        const NodeInfo &ni = h->nodes[j];
+        if (!ni.live()) continue;
+        const float *now = ni.feat.size() == K ? ni.feat.data() : zeros.data();
+        if (j >= snap_n || memcmp(now, s->feat_snap.data() + (size_t)j * K, (size_t)K * 4) != 0) out.push_back(j);
+    }
+    return out;
+}
+
+// The affinity change set of DESIGN.md 3.15: a live node's cost does not depend on its weight, so REPLACE is every interned node not
+// live now and CANDIDATES every changed node live now that was not live before; a live -> live weight change is a no-op.  The
+// refeatured (and, for failure-domain lists, relabelled) live nodes are added as REPLACE | CANDIDATE by the caller.
+ChangeSetHost build_affinity_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
+    const uint32_t n_total = (uint32_t)h->nodes.size();
+    const size_t pad = (n_total + 3) & ~(size_t)3;
+    ChangeSetHost cs;
+    cs.bytes.assign(std::max<size_t>(pad, 4), 0);
+    for (uint32_t j = 0; j < n_total; j++) if (!h->nodes[j].live()) cs.bytes[j] = kChgReplace;
+    std::vector<uint32_t> cand;
+    for (size_t i = 0; i < k; i++)
+        if (h->nodes[idx[i]].live() && !prev_weight[i]) { cs.bytes[idx[i]] = kChgCandidate; cand.push_back(idx[i]); }
+    cs.n_cand = (uint32_t)cand.size();
+    const size_t o = cs.bytes.size();
+    cs.bytes.resize(o + cand.size() * 4);
+    if (!cand.empty()) memcpy(cs.bytes.data() + o, cand.data(), cand.size() * 4);
+    return cs;
+}
+
+// set_assign_ranked_affinity(_spread): fresh lists of the set's features on the path affinity_path() gives now, column 0 into idx,
+// the counters rebuilt from it, and the kind, path, K, node features (and labels) they were computed under recorded
+void set_assign_affinity_lists(rio_objset *s, uint32_t ranks, bool spread) {
+    rio_placement *h = s->h;
+    check_ranked_args(s->n, ranks);
+    REQUIRE(h->K > 0, "assign with object features needs node features");
+    REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+    require_affinity_set_kernels(spread);
+    ensure_tab(h);
+    s->drop_lists();
+    s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
+    set_ensure_counters(s);
+    const AffinityPath path = affinity_path(h);
+    if (s->n) {
+        if (spread) run_affinity_spread(h, s->feats.as<float>(), s->n, ranks, s->lists.as<uint32_t>(), path);
+        else run_affinity_ranked(h, s->feats.as<float>(), s->n, ranks, s->lists.as<uint32_t>(), path);
+    }
+    launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
+    set_zero_counters(s);
+    launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
+    s->assigned = true;
+    s->ranks = ranks;
+    s->rank_solver = h->solver;
+    s->rank_bits = h->trie_bits;
+    s->spread = spread;
+    s->affinity = true;
+    // with no live node the path is decided by what the handle would take for K == 16
+    s->aff_tensor = path == AffinityPath::kTensorCores || (path == AffinityPath::kNoLiveNode && affinity_umma_wanted());
+    s->aff_K = h->K;
+    snapshot_feats(s);
+    if (spread) snapshot_labels(s);
+}
+
+// set_rebalance_changes_ranked on affinity lists (DESIGN.md 3.15): one pass classifies every list (S1 to s->sel, S2 rows merged with
+// the candidates in place), then the S1 rows are recomputed on the recorded path and scattered back
+void rebalance_affinity_lists(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t &moved, uint64_t &changed) {
+    rio_placement *h = s->h;
+    const bool spread = s->spread;
+    const uint32_t R = s->ranks, K = s->aff_K;
+    const std::vector<uint32_t> refeatured = refeatured_live(s);
+    const std::vector<uint32_t> relabelled = spread ? relabelled_live(s) : std::vector<uint32_t>{};
+    if (k || !refeatured.empty() || !relabelled.empty()) {
+        ensure_tab(h);
+        if (spread) ensure_aff_dom(h);
+        set_ensure_counters(s);
+        zero_scalar(h, S_MOVED);
+        zero_scalar(h, S_CHANGED);
+        zero_scalar(h, S_NSEL);
+        ChangeSetHost cs = build_affinity_change_set(h, idx, prev_weight, k);
+        add_relabels(cs, refeatured);
+        add_relabels(cs, relabelled);
+        const ChangeSetDev dcs = upload_change_set(h, cs);
+        uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>();
+        const uint32_t n_total = h->tabs.tab.n_total;
+        launch_rebalance_changes_affinity(h->L(), s->feats.as<float>(), K, lists, R, d_idx, s->n, h->d_fnode.as<float>(), n_total, dcs,
+                                          spread ? h->aff_dom.as<uint32_t>() : nullptr, counters, s->sel.as<uint32_t>(), h->d_scalars + S_NSEL,
+                                          h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
+        const uint64_t n_sel = read_scalar(h, S_NSEL);
+        if (n_sel) {   // S1: the selected objects' lists computed afresh on the recorded path, scattered back
+            h->s_feats.ensure(n_sel * K * 4, h->stream);
+            h->s_idx.ensure(n_sel * R * 4, h->stream);
+            launch_gather_rows(h->L(), s->feats.as<float>(), K, s->sel.as<uint32_t>(), n_sel, h->s_feats.as<float>());
+            const AffinityPath path = affinity_path(h, s->aff_tensor);
+            if (spread) run_affinity_spread(h, h->s_feats.as<float>(), n_sel, R, h->s_idx.as<uint32_t>(), path);
+            else run_affinity_ranked(h, h->s_feats.as<float>(), n_sel, R, h->s_idx.as<uint32_t>(), path);
+            launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel, R, lists, d_idx, counters, n_total, h->d_scalars + S_MOVED,
+                                  h->d_scalars + S_CHANGED);
+        }
+        moved = read_scalar(h, S_MOVED);
+        changed = read_scalar(h, S_CHANGED);
+    }
+    snapshot_feats(s);
+    if (spread) snapshot_labels(s);
+}
+
 }  // namespace
 
 rio_status rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks) {
@@ -2042,6 +2186,16 @@ rio_status rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks) {
 rio_status rio_cuda_set_assign_ranked_spread(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
     return guarded(s->h, [&] { set_assign_lists(s, ranks, true); });
+}
+
+rio_status rio_cuda_set_assign_ranked_affinity(rio_objset *s, uint32_t ranks) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    return guarded(s->h, [&] { set_assign_affinity_lists(s, ranks, false); });
+}
+
+rio_status rio_cuda_set_assign_ranked_affinity_spread(rio_objset *s, uint32_t ranks) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    return guarded(s->h, [&] { set_assign_affinity_lists(s, ranks, true); });
 }
 
 rio_status rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out) {
@@ -2063,9 +2217,18 @@ rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *
     return guarded(h, [&] {
         check_change_set(h, idx, prev_weight, k);
         const bool spread = s->spread;   // the kind of lists the set holds (false when it holds none)
-        if (spread) require_spread_set_kernels(h->solver);
+        if (s->affinity) require_affinity_set_kernels(spread);
+        else if (spread) require_spread_set_kernels(h->solver);
         else require_ranked_set_kernels(h->solver);
         REQUIRE(s->ranks, "set holds no ranked lists");
+        if (s->affinity) {   // affinity lists (DESIGN.md 3.15): the solver and trie_bits play no part
+            REQUIRE(h->K == s->aff_K, "the set's affinity lists were computed under another node feature K: assign the lists again");
+            uint64_t moved = 0, changed = 0;
+            rebalance_affinity_lists(s, idx, prev_weight, k, moved, changed);
+            if (out_moved) *out_moved = moved;
+            if (out_changed) *out_changed = changed;
+            return;
+        }
         REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
         const uint32_t R = s->ranks;
         uint64_t moved = 0, changed = 0;

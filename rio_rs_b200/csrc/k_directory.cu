@@ -423,19 +423,6 @@ __device__ __forceinline__ uint32_t change_target(uint64_t key, uint32_t cur, co
     return best;
 }
 
-// Every lane of the warp calls this with its number of items; returns the position of the lane's first item in a list whose
-// length is *n (one atomic per warp).
-__device__ __forceinline__ unsigned long long warp_reserve(unsigned long long *n, uint32_t mine) {
-    const unsigned lane = threadIdx.x & 31;
-    uint32_t pre = mine;   // inclusive warp prefix sum
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, pre, o); if (lane >= (unsigned)o) pre += t; }
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, pre, 31);
-    unsigned long long b = 0;
-    if (lane == 0 && total) b = atomicAdd(n, (unsigned long long)total);
-    return __shfl_sync(0xFFFFFFFFu, b, 0) + (pre - mine);
-}
-
 // Directory, 16 B/slot stream: four independent 128-bit slot loads per thread per trip.  The trip loop is warp-uniform (the
 // capacity is a power of two >= 1024), so the R1 append can ballot.
 template <bool SMEM>

@@ -1,5 +1,6 @@
-// k_rank_common.cuh -- launch shape, shared-memory staging, the exact HRW2 contest, the compare-mode epilogue and the rank dispatch of
-// the ranked walks (k_ranked.cu, k_spread.cu) and the ranked change-set passes (k_directory.cu).
+// k_rank_common.cuh -- launch shape, shared-memory staging, the exact HRW2 contest, the compare-mode epilogue, the warp-aggregated
+// list append and the rank dispatch of the ranked walks (k_ranked.cu, k_spread.cu) and the change-set passes (k_directory.cu,
+// k_affinity_set.cu).
 // Included by .cu files only: everything is internal to the including translation unit.
 #pragma once
 #include "kernels.cuh"
@@ -61,6 +62,19 @@ __device__ __forceinline__ void spread_insert(uint64_t (&gs)[R], uint32_t (&gu)[
         s = sw ? ts : s; u = sw ? tu : u; j = sw ? tj : j; d = sw ? td : d;
         go = go && !(sw && td == dc);
     }
+}
+
+// Every lane of the warp calls this with its number of items; returns the position of the lane's first item in a list whose
+// length is *n (one atomic per warp).
+__device__ __forceinline__ unsigned long long warp_reserve(unsigned long long *n, uint32_t mine) {
+    const unsigned lane = threadIdx.x & 31;
+    uint32_t pre = mine;   // inclusive warp prefix sum
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, pre, o); if (lane >= (unsigned)o) pre += t; }
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, pre, 31);
+    unsigned long long b = 0;
+    if (lane == 0 && total) b = atomicAdd(n, (unsigned long long)total);
+    return __shfl_sync(0xFFFFFFFFu, b, 0) + (pre - mine);
 }
 
 // Compare mode of the HRW2 walks (DESIGN.md 3.11, 3.13): the output holds the stored lists of a resident set.  Each walk is compared

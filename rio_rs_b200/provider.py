@@ -591,6 +591,19 @@ class ObjectSet:
         self._ck(self.L.rio_cuda_set_assign_ranked_spread(self.s, ranks))
         self._ranks = int(ranks)
 
+    def assign_ranked_affinity(self, ranks):
+        """Each object's `ranks` lowest-cost nodes under the affinity cost of the set's features (load_feats), kept in the set
+        (DESIGN.md 3.15) with the path, K and node features they were computed under.  rebalance_changes_ranked keeps them current,
+        node feature changes since the last call included; load_feats drops them."""
+        self._ck(self.L.rio_cuda_set_assign_ranked_affinity(self.s, ranks))
+        self._ranks = int(ranks)
+
+    def assign_ranked_affinity_spread(self, ranks):
+        """assign_ranked_affinity with each object's `ranks` lowest-cost nodes in distinct failure domains (DESIGN.md 3.15); the labels
+        are recorded too, and relabels since the last call belong to the next change set."""
+        self._ck(self.L.rio_cuda_set_assign_ranked_affinity_spread(self.s, ranks))
+        self._ranks = int(ranks)
+
     def read_ranked(self, first=0, n=None):
         """Rows [first, first + n) of the ranked lists -> (n, ranks) uint32, RIO_NONE past the live set."""
         if n is None:

@@ -100,6 +100,8 @@ extern "C" {
     pub fn rio_cuda_set_rebalance_changes_ranked(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64,
                                                  out_changed: *mut u64) -> rio_status;
     pub fn rio_cuda_set_assign_ranked_spread(s: *mut rio_objset, ranks: u32) -> rio_status;
+    pub fn rio_cuda_set_assign_ranked_affinity(s: *mut rio_objset, ranks: u32) -> rio_status;
+    pub fn rio_cuda_set_assign_ranked_affinity_spread(s: *mut rio_objset, ranks: u32) -> rio_status;
     pub fn rio_cuda_set_counters(s: *mut rio_objset, out: *mut u32, cap: u32) -> rio_status;
     pub fn rio_cuda_set_read(s: *mut rio_objset, first: u64, n: u64, out_keys: *mut u64, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_set_size(s: *mut rio_objset, out_n: *mut u64) -> rio_status;
