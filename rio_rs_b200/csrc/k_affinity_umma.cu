@@ -286,9 +286,10 @@ k_affinity_resolve(const float *__restrict__ fobj, uint64_t n, const float *__re
             const float4 x = __ldg(fn + k * 8);                                 // rows beyond n_live are zero padding
             a = fmaf(o[k].x, x.x, a); a = fmaf(o[k].y, x.y, a); a = fmaf(o[k].z, x.z, a); a = fmaf(o[k].w, x.w, a);
         }
-        // order-preserving integer image of cost = -dot (+inf for padding); minimum of (key, position) over the 8 lanes
+        // order-preserving integer image of cost = -dot (+inf for padding); minimum of (key, position) over the 8 lanes.  `+ 0.f`
+        // turns -0 into +0: the image puts -0 before +0, the float order of the CUDA cores (DESIGN.md 3.6) does not
         uint32_t p = g * 8 + r;
-        const uint32_t bits = p < n_live ? __float_as_uint(-a) : 0x7F800000u;
+        const uint32_t bits = p < n_live ? __float_as_uint(-a + 0.f) : 0x7F800000u;
         int key = (int)(bits ^ ((uint32_t)((int)bits >> 31) & 0x7FFFFFFFu));
         if (p >= n_live) p = kNone;
 #pragma unroll
@@ -494,7 +495,7 @@ k_affinity_resolve_ranked(const float *__restrict__ fobj, uint64_t n, const floa
             }
             uint32_t p = gj * 8 + r;
             const bool live = gj != kNone && p < n_live;
-            const uint32_t bits = live ? __float_as_uint(-a) : 0x7F800000u;
+            const uint32_t bits = live ? __float_as_uint(-a + 0.f) : 0x7F800000u;   // one zero, as in k_affinity_resolve
             key[j] = (int)(bits ^ ((uint32_t)((int)bits >> 31) & 0x7FFFFFFFu));
             pos[j] = live ? p : kNone;
         }
@@ -660,7 +661,7 @@ k_affinity_resolve_spread(const float *__restrict__ fobj, uint64_t n, const floa
             const float4 x = __ldg(fn + k * 8);
             a = fmaf(o[k].x, x.x, a); a = fmaf(o[k].y, x.y, a); a = fmaf(o[k].z, x.z, a); a = fmaf(o[k].w, x.w, a);
         }
-        const uint32_t bits = __float_as_uint(-a);
+        const uint32_t bits = __float_as_uint(-a + 0.f);   // one zero, as in k_affinity_resolve
         return (int)(bits ^ ((uint32_t)((int)bits >> 31) & 0x7FFFFFFFu));
     };
     // smallest (key, position) over the 8 lanes of an object, its domain carried along

@@ -6,6 +6,7 @@
 // the costs are summed exactly as launchers.cpp's launch_assign_affinity sums them, so rank 1 is that double's answer.  Nothing here
 // says anything about the kernels, which are proven on the GPU against the fp64 oracle.
 #include <algorithm>
+#include <cmath>
 #include <utility>
 #include <vector>
 
@@ -24,7 +25,7 @@ void launch_assign_affinity_ranked(const Launch &L, const float *fobj, uint64_t 
         for (uint32_t j = 0; j < n_total; j++) {
             if (!live[j]) continue;
             float acc = 0.f;
-            for (uint32_t k = 0; k < K; k++) acc += fobj[i * K + k] * fnode[(size_t)j * K + k];
+            for (uint32_t k = 0; k < K; k++) acc = std::fmaf(fobj[i * K + k], fnode[(size_t)j * K + k], acc);
             c.emplace_back(-acc, j);
         }
         std::sort(c.begin(), c.end());

@@ -6,6 +6,7 @@
 // the costs are summed exactly as launchers.cpp's launch_assign_affinity sums them, so an S2 row is what the affinity doubles would
 // list.  Nothing here says anything about the kernels, which are proven on the GPU against the fp64 oracle.
 #include <algorithm>
+#include <cmath>
 #include <tuple>
 #include <vector>
 
@@ -32,7 +33,7 @@ void launch_rebalance_changes_affinity(const Launch &L, const float *fobj, uint3
         std::vector<std::tuple<float, uint32_t>> c;
         for (uint32_t j : nodes) {
             float acc = 0.f;
-            for (uint32_t k = 0; k < K; k++) acc += fobj[i * K + k] * fnode[(size_t)j * K + k];
+            for (uint32_t k = 0; k < K; k++) acc = std::fmaf(fobj[i * K + k], fnode[(size_t)j * K + k], acc);
             c.emplace_back(-acc, j);
         }
         std::sort(c.begin(), c.end());

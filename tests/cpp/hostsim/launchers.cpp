@@ -10,6 +10,7 @@
 #include <sched.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstring>
 #include <vector>
 
@@ -147,6 +148,7 @@ void launch_dir_reassign_trie(const Launch &L, const DirDev &dir, const TrieDev 
     count(L);
 }
 
+// c32 of DESIGN.md 3.6: fmaf in k order from 0.f, as every affinity kernel sums (a plain `acc += a * b` is not contracted by g++)
 void launch_assign_affinity(const Launch &L, const float *fobj, uint64_t n, const float *fnode, const uint32_t *live, uint32_t n_total, uint32_t K, uint32_t *out, float *out_cost,
                             uint32_t *counters) {
     if (!n) return;
@@ -156,7 +158,7 @@ void launch_assign_affinity(const Launch &L, const float *fobj, uint64_t n, cons
         for (uint32_t j = 0; j < n_total; j++) {
             if (!live[j]) continue;
             float acc = 0.f;
-            for (uint32_t k = 0; k < K; k++) acc += fobj[i * K + k] * fnode[(size_t)j * K + k];
+            for (uint32_t k = 0; k < K; k++) acc = std::fmaf(fobj[i * K + k], fnode[(size_t)j * K + k], acc);
             const float cost = -acc;
             if (bj == kNone || cost < best) { best = cost; bj = j; }   // ties -> lowest j
         }
