@@ -140,9 +140,17 @@ rio_status  rio_cuda_assign_batch(rio_placement *h, const uint64_t *keys, const 
                                   uint32_t *out_idx);
 /* assign_batch followed by the bounded-load rounds of rio_cuda_set_assign_bounded (DESIGN.md 3.5) for host buffers: the
  * per-node histogram is fused into the score kernels of the chunk pipeline, the counter exchange + capacity check runs on
- * the device behind the last chunk.  n_total = global object count (0 = n * world).  Hash path only. */
+ * the device behind the last chunk.  n_total = global object count (0 = n * world).  Hash path; the affinity cost:
+ * rio_cuda_assign_bounded_affinity_batch. */
 rio_status  rio_cuda_assign_bounded_batch(rio_placement *h, const uint64_t *keys, size_t n, uint64_t n_total, uint32_t cap_num,
                                           uint32_t cap_den, uint32_t max_rounds, uint32_t *out_idx, uint32_t *out_passes);
+/* rio_cuda_set_assign_bounded_affinity for host buffers: keys (n) feed the spill hash, obj_feats (n x K, K of set_nodes) the cost.
+ * Returns exactly what the set call returns for the same keys and features.  Argument rules as for rio_cuda_assign_bounded_batch;
+ * also RIO_ERR_UNKNOWN for NULL buffers or a handle without node features, RIO_ERR_UPSTREAM when the library was built without the
+ * bounded affinity kernels. */
+rio_status  rio_cuda_assign_bounded_affinity_batch(rio_placement *h, const uint64_t *keys, const float *obj_feats, size_t n,
+                                                   uint64_t n_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                                                   uint32_t *out_idx, uint32_t *out_passes);
 /* Ranked placement (DESIGN.md 3.9): each object's first `ranks` distinct nodes under the handle's solver policy.  rank 1 is
  * exactly what assign_batch returns; rank r is the same policy's placement over the live set minus ranks 1..r-1 -- so rank 2 is
  * where a LEAVE of rank 1 sends the object (its failover target).  Pure function of (keys, live set); hash path only (the affinity cost: rio_cuda_assign_ranked_affinity_batch).
@@ -235,6 +243,14 @@ rio_status  rio_cuda_set_assign_bounded(rio_objset *s, uint64_t n_total, uint32_
  * _begin / _end calls in the same order.  rio_cuda_set_assign_bounded == _begin followed by _end. */
 rio_status  rio_cuda_set_assign_bounded_begin(rio_objset *s, uint64_t n_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds);
 rio_status  rio_cuda_set_assign_bounded_end(rio_objset *s, uint32_t *out_passes);
+/* Bounded-load rounds under the affinity cost (DESIGN.md 3.16): the capacities, counters, spill selection and closed set of
+ * rio_cuda_set_assign_bounded, with pass 0 = rio_cuda_set_assign(s, 1) bit for bit, and a spilled object re-placed at its lowest
+ * cost over the live nodes not closed, on the kernel path pass 0 took.  Node weights set the capacities; the costs ignore them.
+ * Needs the set's keys (spill hash) and features (set_load_feats, K of the handle).  Drops ranked lists.  RIO_ERR_UNKNOWN for a
+ * handle without node features, set features missing or of another K, or a bounded call in flight on the set (between _begin and
+ * _end); RIO_ERR_UPSTREAM when the library was built without the bounded affinity kernels. */
+rio_status  rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total, uint32_t cap_num, uint32_t cap_den,
+                                                 uint32_t max_rounds, uint32_t *out_passes);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
 /* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied

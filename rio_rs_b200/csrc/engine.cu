@@ -11,6 +11,7 @@
 #include "k_affinity_ranked.cuh"
 #include "k_affinity_spread.cuh"
 #include "k_affinity_set.cuh"
+#include "k_affinity_bounded.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -177,6 +178,9 @@ struct rio_placement {
     TabBufs tabs, tabs_masked;
     DevBuf d_fnode, d_fnode_c, d_fnode_g, d_nidx_map;
     uint32_t aff_live = 0, aff_pad = 0;   // compacted live-node operands of the tensor-core affinity kernel
+    // the same operands over live minus closed, rebuilt for every spill round of a bounded affinity call (DESIGN.md 3.16); grow-only
+    DevBuf d_fnode_cm, d_fnode_gm, d_nidx_map_m;
+    uint32_t aff_live_m = 0, aff_pad_m = 0;
 
     DirDev dir{};
     uint64_t dir_cap = 0;
@@ -185,6 +189,7 @@ struct rio_placement {
     uint32_t dir_seq = 0;           // upsert sequence numbers handed out so far (ordering of duplicate keys, k_dir_upsert)
 
     DevBuf s_keys, s_idx, s_idx2, s_sel, s_slots, s_keys2, s_feats, s_packed, s_offsets, s_cost, s_misc, s_flush, s_gather;
+    DevBuf s_rows;                            // the spilled objects' feature rows of a bounded affinity round
     // bounded-load state kept on the device between passes (DESIGN.md 3.5): [ticket | cap | global counters | thr | closed epoch | over] x node
     BoundedState bs;                          // for rio_cuda_assign_bounded_batch (host buffers)
     uint64_t tab_version = 0;
@@ -363,7 +368,7 @@ void build_tab(rio_placement *h, TabBufs &tb, const std::vector<uint8_t> *closed
     for (uint32_t j = 0; j < n_total; j++) {
         const NodeInfo &ni = h->nodes[j];
         state[j] = ((ni.active && !ni.malformed) ? kNodeLive : 0) | (ni.malformed ? kNodeMalformed : 0);
-        livef[j] = ni.live() ? 1u : 0u;
+        livef[j] = (ni.live() && !is_closed(j)) ? 1u : 0u;   // the CUDA-core affinity rounds of 3.16 read the masked flags
     }
 
     // ---- one staging area, one copy ----
@@ -410,6 +415,37 @@ uint64_t live_signature(const rio_placement *h) {
     return sig;
 }
 
+// The compacted live nodes (node-index order) of the tensor-core affinity kernel, zero padded to the node tile, without the nodes
+// `closed` marks (a spill round of DESIGN.md 3.16), into (fc, fg, map); n_live / n_pad receive the kernel's live and padded counts.
+// Synchronises the stream: the host vectors go out of scope.
+void build_aff_operands(rio_placement *h, const std::vector<uint8_t> *closed, DevBuf &fc_buf, DevBuf &fg_buf, DevBuf &map_buf, uint32_t &n_live,
+                        uint32_t &n_pad) {
+    const uint32_t n_total = (uint32_t)h->nodes.size();
+    cudaStream_t st = h->stream;
+    auto is_closed = [&](uint32_t j) { return closed && j < closed->size() && (*closed)[j]; };
+    std::vector<uint32_t> map;
+    for (uint32_t j = 0; j < n_total; j++) if (h->nodes[j].live() && !is_closed(j)) map.push_back(j);
+    const uint32_t nl = (uint32_t)map.size();
+    const uint32_t pad = nl <= 64 ? 64 : (nl + 255) / 256 * 256;
+    std::vector<float> fc((size_t)pad * 16, 0.f);
+    for (uint32_t q = 0; q < nl; q++) if (h->nodes[map[q]].feat.size() == 16) std::copy(h->nodes[map[q]].feat.begin(), h->nodes[map[q]].feat.end(), fc.begin() + (size_t)q * 16);
+    map.resize(pad, kNone);
+    // the same rows regrouped as [group of 8 nodes][16-byte piece][node in group] for k_affinity_resolve
+    std::vector<float> fg(fc.size());
+    for (uint32_t g8 = 0; g8 < pad / 8; g8++)
+        for (uint32_t k4 = 0; k4 < 4; k4++)
+            for (uint32_t r8 = 0; r8 < 8; r8++)
+                std::copy_n(fc.begin() + ((size_t)g8 * 8 + r8) * 16 + k4 * 4, 4, fg.begin() + (((size_t)g8 * 4 + k4) * 8 + r8) * 4);
+    fc_buf.ensure(fc.size() * 4, st);
+    fg_buf.ensure(fg.size() * 4, st);
+    CUDA_TRY(cudaMemcpyAsync(fg_buf.p, fg.data(), fg.size() * 4, cudaMemcpyHostToDevice, st));
+    map_buf.ensure(map.size() * 4, st);
+    CUDA_TRY(cudaMemcpyAsync(fc_buf.p, fc.data(), fc.size() * 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(map_buf.p, map.data(), map.size() * 4, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    n_live = nl; n_pad = pad;
+}
+
 void ensure_tab(rio_placement *h) {
     if (!h->tab_dirty) return;
     build_tab(h, h->tabs, nullptr);
@@ -426,31 +462,8 @@ void ensure_tab(rio_placement *h) {
     }
     h->d_fnode.ensure(fnode.size() * 4, st);
     CUDA_TRY(cudaMemcpyAsync(h->d_fnode.p, fnode.data(), fnode.size() * 4, cudaMemcpyHostToDevice, st));
-    // compacted live nodes (node-index order) for the tensor-core affinity kernel, zero padded to the node tile
     h->aff_live = h->aff_pad = 0;
-    if (h->K == 16) {
-        std::vector<uint32_t> map;
-        for (uint32_t j = 0; j < n_total; j++) if (h->nodes[j].live()) map.push_back(j);
-        const uint32_t nl = (uint32_t)map.size();
-        const uint32_t pad = nl <= 64 ? 64 : (nl + 255) / 256 * 256;
-        std::vector<float> fc((size_t)pad * 16, 0.f);
-        for (uint32_t q = 0; q < nl; q++) if (h->nodes[map[q]].feat.size() == 16) std::copy(h->nodes[map[q]].feat.begin(), h->nodes[map[q]].feat.end(), fc.begin() + (size_t)q * 16);
-        map.resize(pad, kNone);
-        // the same rows regrouped as [group of 8 nodes][16-byte piece][node in group] for k_affinity_resolve
-        std::vector<float> fg(fc.size());
-        for (uint32_t g8 = 0; g8 < pad / 8; g8++)
-            for (uint32_t k4 = 0; k4 < 4; k4++)
-                for (uint32_t r8 = 0; r8 < 8; r8++)
-                    std::copy_n(fc.begin() + ((size_t)g8 * 8 + r8) * 16 + k4 * 4, 4, fg.begin() + (((size_t)g8 * 4 + k4) * 8 + r8) * 4);
-        h->d_fnode_c.ensure(fc.size() * 4, st);
-        h->d_fnode_g.ensure(fg.size() * 4, st);
-        CUDA_TRY(cudaMemcpyAsync(h->d_fnode_g.p, fg.data(), fg.size() * 4, cudaMemcpyHostToDevice, st));
-        h->d_nidx_map.ensure(map.size() * 4, st);
-        CUDA_TRY(cudaMemcpyAsync(h->d_fnode_c.p, fc.data(), fc.size() * 4, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaMemcpyAsync(h->d_nidx_map.p, map.data(), map.size() * 4, cudaMemcpyHostToDevice, st));
-        CUDA_TRY(cudaStreamSynchronize(st));
-        h->aff_live = nl; h->aff_pad = pad;
-    }
+    if (h->K == 16) build_aff_operands(h, nullptr, h->d_fnode_c, h->d_fnode_g, h->d_nidx_map, h->aff_live, h->aff_pad);
     CUDA_TRY(cudaStreamSynchronize(st));   // the host vectors above go out of scope
 }
 
@@ -683,9 +696,9 @@ AffinityPath affinity_path(const rio_placement *h, bool want_umma = affinity_umm
     return AffinityPath::kCudaCores;
 }
 
-void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d_out_idx, float *d_out_cost, uint32_t *d_counters) {
+void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d_out_idx, float *d_out_cost, uint32_t *d_counters, AffinityPath path) {
     if (!n) return;
-    switch (affinity_path(h)) {
+    switch (path) {
         case AffinityPath::kNoLiveNode: launch_fill_u32(h->L(), d_out_idx, n, kNone); break;
         case AffinityPath::kTensorCores:
             CUDA_TRY(launch_assign_affinity_umma(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(), h->aff_live,
@@ -798,7 +811,7 @@ void assign_host_pipelined(rio_placement *h, const uint64_t *keys, const float *
         CUDA_TRY(cudaEventRecord(h->ev_pipe[1], h->h2d_stream));
         CUDA_TRY(cudaStreamWaitEvent(h->stream, h->ev_pipe[1], 0));
         if (feats)
-            run_affinity(h, h->s_feats.as<float>() + lo * h->K, m, h->s_idx.as<uint32_t>() + lo, nullptr, nullptr);
+            run_affinity(h, h->s_feats.as<float>() + lo * h->K, m, h->s_idx.as<uint32_t>() + lo, nullptr, nullptr, affinity_path(h));
         else
             run_assign(h, h->solver, h->tabs, h->s_keys.as<uint64_t>() + lo, m, h->s_idx.as<uint32_t>() + lo, d_counters, nullptr, 0);
         CUDA_TRY(cudaEventRecord(h->ev_pipe[2], h->stream));
@@ -964,7 +977,11 @@ void bounded_begin(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, u
 }
 
 // Second half: wait for the check (two words in mapped memory), run the spill rounds it asks for.  Returns the passes run.
-uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, uint64_t n, uint32_t *d_idx, uint32_t *d_counters, uint32_t *d_sel) {
+// replace(closed, nsel) re-places the nsel objects of d_sel over live minus closed, adding them to d_counters: hash_replace for the
+// hash policy, the affinity launch of the call's path for 3.16.
+template <class Replace>
+uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, uint64_t n, uint32_t *d_idx, uint32_t *d_counters, uint32_t *d_sel,
+                     Replace &&replace) {
     REQUIRE(bs.active, "no bounded call in flight on this set");
     bs.active = false;
     cudaStream_t st = h->stream;
@@ -985,12 +1002,54 @@ uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys,
         const uint64_t nsel = read_scalar(h, S_NSEL);
         std::vector<uint8_t> closed(M, 0);
         for (uint32_t j = 0; j < M; j++) closed[j] = ce[j] == bs.epoch;
-        build_tab(h, h->tabs_masked, &closed);
-        if (nsel) run_assign(h, h->solver, h->tabs_masked, d_keys, n, d_idx, d_counters, d_sel, nsel);
+        replace(closed, nsel);
         passes++;
         if (r + 1 < bs.max_rounds) { order_behind_aux_checks(h); launch_check(h, bs, d_counters, b, M, nullptr, st); }
     }
     return passes;
+}
+
+// the spill rounds of 3.5: the handle's policy over the masked table
+auto hash_replace(rio_placement *h, const uint64_t *d_keys, uint64_t n, uint32_t *d_idx, uint32_t *d_counters, uint32_t *d_sel) {
+    return [=](const std::vector<uint8_t> &closed, uint64_t nsel) {
+        build_tab(h, h->tabs_masked, &closed);
+        if (nsel) run_assign(h, h->solver, h->tabs_masked, d_keys, n, d_idx, d_counters, d_sel, nsel);
+    };
+}
+
+// ---- bounded-load rounds under the affinity cost (DESIGN.md 3.16) ----------------------------------------------------------------
+void require_bounded_affinity_kernels() {
+    if (!launch_scatter_idx || !launch_gather_rows)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no bounded affinity kernels (k_affinity_bounded.cuh launchers are not linked)"};
+}
+
+// Pass 0 is run_affinity with the counters on the path affinity_path() gives now, then the rounds of 3.5.  A round re-places its
+// spilled objects on the same path over live minus closed: the CUDA-core kernel with the masked table's live flags, or the tensor-core
+// kernel over operands compacted without the closed nodes.  The rows go through s_rows, the new nodes through s_idx2.
+uint32_t bounded_affinity(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, uint64_t n, uint32_t *d_idx, uint32_t *d_counters,
+                          uint32_t M, uint32_t *d_sel, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds) {
+    const AffinityPath path = affinity_path(h);
+    const uint32_t K = h->K, n_total = h->tabs.tab.n_total;
+    CUDA_TRY(cudaMemsetAsync(d_counters, 0, (size_t)std::max(M, 1u) * 4, h->stream));
+    run_affinity(h, d_feats, n, d_idx, nullptr, d_counters, path);
+    bounded_begin(h, bs, d_keys, n, d_idx, d_counters, M, n_total_objs, cap_num, cap_den, max_rounds, true, true, nullptr);
+    return bounded_end(h, bs, d_keys, n, d_idx, d_counters, d_sel, [&](const std::vector<uint8_t> &closed, uint64_t nsel) {
+        if (path == AffinityPath::kTensorCores) build_aff_operands(h, &closed, h->d_fnode_cm, h->d_fnode_gm, h->d_nidx_map_m, h->aff_live_m, h->aff_pad_m);
+        else build_tab(h, h->tabs_masked, &closed);
+        if (!nsel) return;
+        h->s_rows.ensure(nsel * K * 4, h->stream);
+        h->s_idx2.ensure(nsel * 4, h->stream);
+        uint32_t *d_new = h->s_idx2.as<uint32_t>();
+        launch_gather_rows(h->L(), d_feats, K, d_sel, nsel, h->s_rows.as<float>());
+        if (path == AffinityPath::kCudaCores)
+            launch_assign_affinity(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode.as<float>(), h->tabs_masked.live, n_total, K, d_new, nullptr, d_counters);
+        else if (path == AffinityPath::kTensorCores && h->aff_live_m)
+            CUDA_TRY(launch_assign_affinity_umma(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode_cm.as<float>(), h->d_fnode_gm.as<float>(),
+                                                 h->d_nidx_map_m.as<uint32_t>(), h->aff_live_m, h->aff_pad_m, n_total, d_new, nullptr, d_counters));
+        else   // no live node is open (only an active node of weight 0 kept the round going)
+            launch_fill_u32(h->L(), d_new, nsel, kNone);
+        launch_scatter_idx(h->L(), d_new, d_sel, nsel, d_idx);
+    });
 }
 
 template <class F>
@@ -1126,8 +1185,8 @@ void rio_cuda_destroy(rio_placement *h) {
         cudaFree(h->xchg_mine);
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
-    DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->rank_dev, &h->spread_dev, &h->aff_dom};
+    DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->d_fnode_cm, &h->d_fnode_gm, &h->d_nidx_map_m, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->rank_dev, &h->spread_dev, &h->aff_dom};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -1434,12 +1493,43 @@ rio_status rio_cuda_assign_bounded_batch(rio_placement *h, const uint64_t *keys,
         // indices are still crossing PCIe
         assign_host_pipelined(h, keys, nullptr, n, out_idx, d_cnt, false);
         bounded_begin(h, h->bs, h->s_keys.as<uint64_t>(), n, h->s_idx.as<uint32_t>(), d_cnt, M, n_total_objs, cap_num, cap_den, max_rounds, true, true, nullptr);
-        const uint32_t passes = bounded_end(h, h->bs, h->s_keys.as<uint64_t>(), n, h->s_idx.as<uint32_t>(), d_cnt, h->s_sel.as<uint32_t>());
+        const uint32_t passes = bounded_end(h, h->bs, h->s_keys.as<uint64_t>(), n, h->s_idx.as<uint32_t>(), d_cnt, h->s_sel.as<uint32_t>(),
+                                            hash_replace(h, h->s_keys.as<uint64_t>(), n, h->s_idx.as<uint32_t>(), d_cnt, h->s_sel.as<uint32_t>()));
         CUDA_TRY(cudaStreamSynchronize(h->d2h_stream));
         if (passes > 1) {   // a spill round rewrote some indices after their chunk had left: send the final state again
             CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * 4, cudaMemcpyDeviceToHost, h->stream));
             CUDA_TRY(cudaStreamSynchronize(h->stream));
         }
+        if (out_passes) *out_passes = passes;
+    });
+}
+
+rio_status rio_cuda_assign_bounded_affinity_batch(rio_placement *h, const uint64_t *keys, const float *obj_feats, size_t n, uint64_t n_total_objs,
+                                                  uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, uint32_t *out_idx, uint32_t *out_passes) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        if (out_passes) *out_passes = 0;
+        if (!n) return;
+        REQUIRE(keys && obj_feats && out_idx, "null buffer");
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(n < 0xFFFFFFFFull, "batch too large");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        require_bounded_affinity_kernels();
+        ensure_tab(h);
+        const uint32_t M = h->tabs.tab.n_total, K = h->K;
+        if (!n_total_objs) n_total_objs = (uint64_t)n * (uint64_t)h->world;
+        cudaStream_t st = h->stream;
+        h->s_keys.ensure(n * 8, st);
+        h->s_feats.ensure(n * (size_t)K * 4, st);
+        h->s_idx.ensure(n * 4, st);
+        h->s_sel.ensure(n * 4, st);
+        h->s_misc.ensure((size_t)std::max(M, 1u) * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, obj_feats, n * (size_t)K * 4, cudaMemcpyHostToDevice, st));
+        const uint32_t passes = bounded_affinity(h, h->bs, h->s_keys.as<uint64_t>(), h->s_feats.as<float>(), n, h->s_idx.as<uint32_t>(), h->s_misc.as<uint32_t>(), M,
+                                                 h->s_sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds);
+        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
         if (out_passes) *out_passes = passes;
     });
 }
@@ -1452,7 +1542,7 @@ rio_status rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, c
         ensure_tab(h);
         if (d_obj_feats) {
             REQUIRE(h->K > 0, "assign with object features needs node features");
-            run_affinity(h, d_obj_feats, n, d_out_idx, nullptr, nullptr);
+            run_affinity(h, d_obj_feats, n, d_out_idx, nullptr, nullptr, affinity_path(h));
         } else {
             run_assign(h, h->solver, h->tabs, d_keys, n, d_out_idx, nullptr, nullptr, 0);
         }
@@ -1865,7 +1955,7 @@ rio_status rio_cuda_set_assign(rio_objset *s, uint32_t use_affinity) {
         set_zero_counters(s);
         if (use_affinity) {
             REQUIRE(s->K > 0 && s->K == h->K, "set features / node features missing or of different K");
-            run_affinity(h, s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), nullptr, s->counters.as<uint32_t>());
+            run_affinity(h, s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), nullptr, s->counters.as<uint32_t>(), affinity_path(h));
         } else {
             run_assign(h, h->solver, h->tabs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), nullptr, 0);
         }
@@ -1889,7 +1979,8 @@ static void set_bounded_begin(rio_objset *s, uint64_t n_total_objs, uint32_t cap
 }
 static uint32_t set_bounded_end(rio_objset *s) {
     rio_placement *h = s->h;
-    const uint32_t passes = bounded_end(h, s->bs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->sel.as<uint32_t>());
+    const uint32_t passes = bounded_end(h, s->bs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->sel.as<uint32_t>(),
+                                        hash_replace(h, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->sel.as<uint32_t>()));
     s->assigned = true;
     if (s->bs.max_rounds == 1) CUDA_TRY(cudaStreamSynchronize(h->stream));   // otherwise the check's report already ordered the pass before this return
     return passes;
@@ -1913,6 +2004,28 @@ rio_status rio_cuda_set_assign_bounded_end(rio_objset *s, uint32_t *out_passes) 
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
     return guarded(s->h, [&] {
         const uint32_t passes = set_bounded_end(s);
+        if (out_passes) *out_passes = passes;
+    });
+}
+
+rio_status rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                                                uint32_t *out_passes) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+        REQUIRE(!s->bs.active, "a bounded call is already in flight on this set (call _end first)");
+        require_bounded_affinity_kernels();
+        s->drop_lists();
+        ensure_tab(h);
+        set_ensure_counters(s);
+        if (!n_total_objs) n_total_objs = s->n * (uint64_t)h->world;
+        const uint32_t passes = bounded_affinity(h, s->bs, s->keys.as<uint64_t>(), s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(),
+                                                 s->counters_n, s->sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds);
+        s->assigned = true;
+        if (max_rounds == 1) CUDA_TRY(cudaStreamSynchronize(h->stream));   // otherwise the check's report already ordered the pass before this return
         if (out_passes) *out_passes = passes;
     });
 }

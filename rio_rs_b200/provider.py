@@ -335,6 +335,18 @@ class GpuObjectPlacement:
         self._ck(self.L.rio_cuda_assign_bounded_batch(self.h, _ptr(keys), len(keys), n_total, cap_num, cap_den, max_rounds, _ptr(out), C.byref(passes)))
         return out, passes.value
 
+    def assign_bounded_affinity_batch(self, keys, obj_feats, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """assign_batch(obj_feats) + bounded-load rounds (DESIGN.md 3.16) for host buffers: the keys feed the spill hash, the features
+        the cost; returns (indices, passes), what ObjectSet.assign_bounded_affinity gives for the same keys and features."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        obj_feats = np.ascontiguousarray(obj_feats, dtype=np.float32)
+        assert obj_feats.ndim == 2 and len(obj_feats) == len(keys)
+        out = np.empty(len(keys), dtype=np.uint32)
+        passes = C.c_uint32(0)
+        self._ck(self.L.rio_cuda_assign_bounded_affinity_batch(self.h, _ptr(keys), _ptr(obj_feats), len(keys), n_total, cap_num, cap_den, max_rounds, _ptr(out),
+                                                               C.byref(passes)))
+        return out, passes.value
+
     def place_batch(self, keys, policy="hrw", self_address=None):
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
         out = np.empty(len(keys), dtype=np.uint32)
@@ -557,6 +569,12 @@ class ObjectSet:
     def assign_bounded(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
         passes = C.c_uint32(0)
         self._ck(self.L.rio_cuda_set_assign_bounded(self.s, n_total, cap_num, cap_den, max_rounds, C.byref(passes)))
+        return passes.value
+
+    def assign_bounded_affinity(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """Bounded-load rounds under the affinity cost of the set's features (load_feats; DESIGN.md 3.16); returns the passes run."""
+        passes = C.c_uint32(0)
+        self._ck(self.L.rio_cuda_set_assign_bounded_affinity(self.s, n_total, cap_num, cap_den, max_rounds, C.byref(passes)))
         return passes.value
 
     def assign_bounded_begin(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):

@@ -61,6 +61,7 @@ extern "C" {
     pub fn rio_cuda_node_address(h: *mut rio_placement, idx: u32, buf: *mut c_char, cap: size_t, out_len: *mut size_t) -> rio_status;
     pub fn rio_cuda_node_count(h: *mut rio_placement, out_total: *mut u32, out_live: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_bounded_batch(h: *mut rio_placement, keys: *const u64, n: usize, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_bounded_affinity_batch(h: *mut rio_placement, keys: *const u64, obj_feats: *const f32, n: usize, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_check_address_batch(h: *mut rio_placement, addr_idx: *const u32, n: usize, self_idx: u32, out_verdict: *mut u8, out_cleaned: *mut u64) -> rio_status;
     pub fn rio_cuda_node_state(h: *mut rio_placement, idx: u32, active: *mut i32, weight: *mut u32, malformed: *mut i32) -> rio_status;
     pub fn rio_cuda_node_set_domains(h: *mut rio_placement, idx: *const u32, domain: *const u32, k: size_t) -> rio_status;
@@ -93,6 +94,7 @@ extern "C" {
     pub fn rio_cuda_set_assign_bounded(s: *mut rio_objset, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_assign_bounded_begin(s: *mut rio_objset, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32) -> rio_status;
     pub fn rio_cuda_set_assign_bounded_end(s: *mut rio_objset, out_passes: *mut u32) -> rio_status;
+    pub fn rio_cuda_set_assign_bounded_affinity(s: *mut rio_objset, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_rebalance(s: *mut rio_objset, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_rebalance_changes(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_assign_ranked(s: *mut rio_objset, ranks: u32) -> rio_status;
