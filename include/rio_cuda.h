@@ -251,6 +251,21 @@ rio_status  rio_cuda_set_assign_bounded_end(rio_objset *s, uint32_t *out_passes)
  * _end); RIO_ERR_UPSTREAM when the library was built without the bounded affinity kernels. */
 rio_status  rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total, uint32_t cap_num, uint32_t cap_den,
                                                  uint32_t max_rounds, uint32_t *out_passes);
+/* Keeps a bounded-load affinity assignment within capacity through a change set (DESIGN.md 3.17), a change set as
+ * rio_cuda_set_rebalance_changes takes (call AFTER the node table changed).  Pass 0: an object on a node that is not live, was
+ * refeatured since the last call, or is past the table (or on none) is re-placed at its lowest cost over the live set on the path
+ * the set recorded; any other object goes to the lowest-cost node of {its node} u {joined and refeatured live nodes}.  Then the
+ * capacity rounds of rio_cuda_set_assign_bounded_affinity run from those counters, with capacities from n_total (0 = n * world),
+ * cap_num / cap_den and the current live weights.  An object changes node only if pass 0 re-placed it, a candidate beat its node, or
+ * it spilled from a node over capacity; the result is not a fresh bounded call.  out_moved (may be NULL) receives the objects whose
+ * node differs from the one before the call, out_passes (may be NULL) 1 + the rounds run.  Needs the record a successful
+ * rio_cuda_set_assign_bounded_affinity (or this call) leaves; every call that drops ranked lists, and set_load_feats, removes it.
+ * RIO_ERR_UNKNOWN (nothing changed): no record, a handle K other than the recorded one, set features missing or of another K, the
+ * argument errors of rio_cuda_set_rebalance_changes, cap_den == 0, max_rounds == 0, or a bounded call in flight on the set;
+ * RIO_ERR_UPSTREAM when the library was built without the kernels of this call. */
+rio_status  rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k,
+                                                            uint64_t n_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                                                            uint64_t *out_moved, uint32_t *out_passes);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
 /* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied

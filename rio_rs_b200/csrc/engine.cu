@@ -12,6 +12,7 @@
 #include "k_affinity_spread.cuh"
 #include "k_affinity_set.cuh"
 #include "k_affinity_bounded.cuh"
+#include "k_set_bounded_affinity.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -260,7 +261,10 @@ struct rio_objset {
     uint32_t aff_K = 0;
     std::vector<float> feat_snap;
     uint64_t feat_snap_version = 0;
-    void drop_lists() { ranks = 0; spread = false; affinity = false; }
+    // bounded-load affinity record (DESIGN.md 3.17): idx is the result of set_assign_bounded_affinity or of the change-set call that
+    // keeps it, on the path of aff_tensor under aff_K, with the node features of feat_snap.  Cleared with the lists and by load_feats.
+    bool bounded_aff = false;
+    void drop_lists() { ranks = 0; spread = false; affinity = false; bounded_aff = false; }
 };
 
 namespace {
@@ -1023,32 +1027,43 @@ void require_bounded_affinity_kernels() {
         throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no bounded affinity kernels (k_affinity_bounded.cuh launchers are not linked)"};
 }
 
-// Pass 0 is run_affinity with the counters on the path affinity_path() gives now, then the rounds of 3.5.  A round re-places its
-// spilled objects on the same path over live minus closed: the CUDA-core kernel with the masked table's live flags, or the tensor-core
-// kernel over operands compacted without the closed nodes.  The rows go through s_rows, the new nodes through s_idx2.
-uint32_t bounded_affinity(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, uint64_t n, uint32_t *d_idx, uint32_t *d_counters,
-                          uint32_t M, uint32_t *d_sel, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds) {
-    const AffinityPath path = affinity_path(h);
+// Re-places the nsel objects of d_sel on `path`, adding them to d_counters: with closed (a bounded round) over live minus closed -- the
+// CUDA-core kernel with the masked table's live flags, or the tensor-core kernel over operands compacted without the closed nodes --,
+// without (the S1 objects of 3.17) over the live set, as run_affinity places them.  The rows go through s_rows, the new nodes through
+// s_idx2, and k_scatter_idx writes them into d_idx.
+void affinity_replace(rio_placement *h, AffinityPath path, const std::vector<uint8_t> *closed, const float *d_feats, const uint32_t *d_sel, uint64_t nsel,
+                      uint32_t *d_idx, uint32_t *d_counters) {
     const uint32_t K = h->K, n_total = h->tabs.tab.n_total;
+    if (closed) {
+        if (path == AffinityPath::kTensorCores) build_aff_operands(h, closed, h->d_fnode_cm, h->d_fnode_gm, h->d_nidx_map_m, h->aff_live_m, h->aff_pad_m);
+        else build_tab(h, h->tabs_masked, closed);
+    }
+    if (!nsel) return;
+    h->s_rows.ensure(nsel * K * 4, h->stream);
+    h->s_idx2.ensure(nsel * 4, h->stream);
+    uint32_t *d_new = h->s_idx2.as<uint32_t>();
+    launch_gather_rows(h->L(), d_feats, K, d_sel, nsel, h->s_rows.as<float>());
+    if (!closed)
+        run_affinity(h, h->s_rows.as<float>(), nsel, d_new, nullptr, d_counters, path);
+    else if (path == AffinityPath::kCudaCores)
+        launch_assign_affinity(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode.as<float>(), h->tabs_masked.live, n_total, K, d_new, nullptr, d_counters);
+    else if (path == AffinityPath::kTensorCores && h->aff_live_m)
+        CUDA_TRY(launch_assign_affinity_umma(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode_cm.as<float>(), h->d_fnode_gm.as<float>(),
+                                             h->d_nidx_map_m.as<uint32_t>(), h->aff_live_m, h->aff_pad_m, n_total, d_new, nullptr, d_counters));
+    else   // no live node is open (only an active node of weight 0 kept the round going)
+        launch_fill_u32(h->L(), d_new, nsel, kNone);
+    launch_scatter_idx(h->L(), d_new, d_sel, nsel, d_idx);
+}
+
+// Pass 0 is run_affinity with the counters on `path` (affinity_path() now), then the rounds of 3.5, whose spilled objects
+// affinity_replace puts back on the same path over live minus closed.
+uint32_t bounded_affinity(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, uint64_t n, uint32_t *d_idx, uint32_t *d_counters,
+                          uint32_t M, uint32_t *d_sel, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, AffinityPath path) {
     CUDA_TRY(cudaMemsetAsync(d_counters, 0, (size_t)std::max(M, 1u) * 4, h->stream));
     run_affinity(h, d_feats, n, d_idx, nullptr, d_counters, path);
     bounded_begin(h, bs, d_keys, n, d_idx, d_counters, M, n_total_objs, cap_num, cap_den, max_rounds, true, true, nullptr);
     return bounded_end(h, bs, d_keys, n, d_idx, d_counters, d_sel, [&](const std::vector<uint8_t> &closed, uint64_t nsel) {
-        if (path == AffinityPath::kTensorCores) build_aff_operands(h, &closed, h->d_fnode_cm, h->d_fnode_gm, h->d_nidx_map_m, h->aff_live_m, h->aff_pad_m);
-        else build_tab(h, h->tabs_masked, &closed);
-        if (!nsel) return;
-        h->s_rows.ensure(nsel * K * 4, h->stream);
-        h->s_idx2.ensure(nsel * 4, h->stream);
-        uint32_t *d_new = h->s_idx2.as<uint32_t>();
-        launch_gather_rows(h->L(), d_feats, K, d_sel, nsel, h->s_rows.as<float>());
-        if (path == AffinityPath::kCudaCores)
-            launch_assign_affinity(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode.as<float>(), h->tabs_masked.live, n_total, K, d_new, nullptr, d_counters);
-        else if (path == AffinityPath::kTensorCores && h->aff_live_m)
-            CUDA_TRY(launch_assign_affinity_umma(h->L(), h->s_rows.as<float>(), nsel, h->d_fnode_cm.as<float>(), h->d_fnode_gm.as<float>(),
-                                                 h->d_nidx_map_m.as<uint32_t>(), h->aff_live_m, h->aff_pad_m, n_total, d_new, nullptr, d_counters));
-        else   // no live node is open (only an active node of weight 0 kept the round going)
-            launch_fill_u32(h->L(), d_new, nsel, kNone);
-        launch_scatter_idx(h->L(), d_new, d_sel, nsel, d_idx);
+        affinity_replace(h, path, &closed, d_feats, d_sel, nsel, d_idx, d_counters);
     });
 }
 
@@ -1527,7 +1542,7 @@ rio_status rio_cuda_assign_bounded_affinity_batch(rio_placement *h, const uint64
         CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, obj_feats, n * (size_t)K * 4, cudaMemcpyHostToDevice, st));
         const uint32_t passes = bounded_affinity(h, h->bs, h->s_keys.as<uint64_t>(), h->s_feats.as<float>(), n, h->s_idx.as<uint32_t>(), h->s_misc.as<uint32_t>(), M,
-                                                 h->s_sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds);
+                                                 h->s_sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds, affinity_path(h));
         CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * 4, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         if (out_passes) *out_passes = passes;
@@ -1941,6 +1956,7 @@ rio_status rio_cuda_set_load_feats(rio_objset *s, const float *feats, uint32_t K
         CUDA_TRY(cudaMemcpyAsync(s->feats.p, feats, s->n * (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
         s->K = K;
         if (s->affinity) s->drop_lists();   // affinity lists are lists of the features just replaced; hash lists stay
+        s->bounded_aff = false;
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
@@ -2008,6 +2024,10 @@ rio_status rio_cuda_set_assign_bounded_end(rio_objset *s, uint32_t *out_passes) 
     });
 }
 
+namespace {
+void record_affinity(rio_objset *s, AffinityPath path);
+}  // namespace
+
 rio_status rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total_objs, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
                                                 uint32_t *out_passes) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
@@ -2022,10 +2042,13 @@ rio_status rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total_
         ensure_tab(h);
         set_ensure_counters(s);
         if (!n_total_objs) n_total_objs = s->n * (uint64_t)h->world;
+        const AffinityPath path = affinity_path(h);
         const uint32_t passes = bounded_affinity(h, s->bs, s->keys.as<uint64_t>(), s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(),
-                                                 s->counters_n, s->sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds);
+                                                 s->counters_n, s->sel.as<uint32_t>(), n_total_objs, cap_num, cap_den, max_rounds, path);
         s->assigned = true;
         if (max_rounds == 1) CUDA_TRY(cudaStreamSynchronize(h->stream));   // otherwise the check's report already ordered the pass before this return
+        record_affinity(s, path);
+        s->bounded_aff = true;
         if (out_passes) *out_passes = passes;
     });
 }
@@ -2178,6 +2201,14 @@ void snapshot_feats(rio_objset *s) {
     s->feat_snap_version = h->feat_version;
 }
 
+// the path, the handle's K and the node features a set's affinity result was computed under (the lists of 3.15, the bounded record of
+// 3.17); with no live node the path is decided by what the handle would take for K == 16
+void record_affinity(rio_objset *s, AffinityPath path) {
+    s->aff_tensor = path == AffinityPath::kTensorCores || (path == AffinityPath::kNoLiveNode && affinity_umma_wanted());
+    s->aff_K = s->h->K;
+    snapshot_feats(s);
+}
+
 // live nodes whose feature row differs bitwise from the set's snapshot; a node interned after the snapshot counts as refeatured
 std::vector<uint32_t> refeatured_live(const rio_objset *s) {
     const rio_placement *h = s->h;
@@ -2240,10 +2271,7 @@ void set_assign_affinity_lists(rio_objset *s, uint32_t ranks, bool spread) {
     s->rank_bits = h->trie_bits;
     s->spread = spread;
     s->affinity = true;
-    // with no live node the path is decided by what the handle would take for K == 16
-    s->aff_tensor = path == AffinityPath::kTensorCores || (path == AffinityPath::kNoLiveNode && affinity_umma_wanted());
-    s->aff_K = h->K;
-    snapshot_feats(s);
+    record_affinity(s, path);
     if (spread) snapshot_labels(s);
 }
 
@@ -2391,6 +2419,54 @@ rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *
         if (spread) snapshot_labels(s);
         if (out_moved) *out_moved = moved;
         if (out_changed) *out_changed = changed;
+    });
+}
+
+// ---- bounded-load affinity sets kept through change sets (DESIGN.md 3.17) ---------------------------------------------------------
+rio_status rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t n_total,
+                                                          uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, uint64_t *out_moved, uint32_t *out_passes) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(s->bounded_aff, "set holds no bounded affinity assignment (set_assign_bounded_affinity first)");
+        REQUIRE(h->K == s->aff_K, "the set's bounded affinity assignment was computed under another node feature K: assign it again");
+        REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+        check_change_set(h, idx, prev_weight, k);
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(!s->bs.active, "a bounded call is already in flight on this set (call _end first)");
+        require_bounded_affinity_kernels();
+        if (!launch_rebalance_changes_bounded_affinity || !launch_count_diff)
+            throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no bounded affinity change-set kernels (k_set_bounded_affinity.cuh launchers are not linked)"};
+        ensure_tab(h);
+        set_ensure_counters(s);   // a join may have interned a node
+        const uint64_t n = s->n;
+        const uint32_t K = s->aff_K, n_total_nodes = h->tabs.tab.n_total;
+        uint32_t *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>(), *d_sel = s->sel.as<uint32_t>();
+        const float *d_feats = s->feats.as<float>();
+        // pass 0: the change set of 3.15 (refeatured live nodes as REPLACE | CANDIDATE), S2 in place, S1 re-placed over the live set
+        ChangeSetHost cs = build_affinity_change_set(h, idx, prev_weight, k);
+        add_relabels(cs, refeatured_live(s));
+        const ChangeSetDev dcs = upload_change_set(h, cs);
+        const AffinityPath path = affinity_path(h, s->aff_tensor);
+        h->s_idx.ensure(std::max<uint64_t>(n, 1) * 4, h->stream);   // each object's node before the call
+        uint32_t *d_prev = h->s_idx.as<uint32_t>();
+        zero_scalar(h, S_NSEL);
+        launch_rebalance_changes_bounded_affinity(h->L(), d_feats, K, d_idx, d_prev, n, h->d_fnode.as<float>(), n_total_nodes, dcs, counters, d_sel,
+                                                  h->d_scalars + S_NSEL);
+        const uint64_t n_sel = read_scalar(h, S_NSEL);
+        affinity_replace(h, path, nullptr, d_feats, d_sel, n_sel, d_idx, counters);
+        // the rounds of 3.16 from the counters pass 0 left, spilled objects re-placed on the same path
+        if (!n_total) n_total = n * (uint64_t)h->world;
+        bounded_begin(h, s->bs, s->keys.as<uint64_t>(), n, d_idx, counters, s->counters_n, n_total, cap_num, cap_den, max_rounds, true, true, nullptr);
+        const uint32_t passes = bounded_end(h, s->bs, s->keys.as<uint64_t>(), n, d_idx, counters, d_sel, [&](const std::vector<uint8_t> &closed, uint64_t nsel) {
+            affinity_replace(h, path, &closed, d_feats, d_sel, nsel, d_idx, counters);
+        });
+        zero_scalar(h, S_MOVED);
+        launch_count_diff(h->L(), d_idx, d_prev, n, h->d_scalars + S_MOVED);
+        const uint64_t moved = read_scalar(h, S_MOVED);
+        snapshot_feats(s);
+        if (out_moved) *out_moved = moved;
+        if (out_passes) *out_passes = passes;
     });
 }
 

@@ -577,6 +577,17 @@ class ObjectSet:
         self._ck(self.L.rio_cuda_set_assign_bounded_affinity(self.s, n_total, cap_num, cap_den, max_rounds, C.byref(passes)))
         return passes.value
 
+    def rebalance_changes_bounded_affinity(self, idx, prev_weight, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """Keeps the assignment of assign_bounded_affinity within capacity after a change set (DESIGN.md 3.17): one change-set pass,
+        then the capacity rounds from the current assignment.  Returns (moved, passes): objects whose node changed, and 1 + the rounds
+        run.  Calls that drop ranked lists, and load_feats, end the set's record; the call then refuses until the next
+        assign_bounded_affinity."""
+        idx, prev = _change_set(idx, prev_weight)
+        m, passes = C.c_uint64(0), C.c_uint32(0)
+        self._ck(self.L.rio_cuda_set_rebalance_changes_bounded_affinity(self.s, _ptr(idx), _ptr(prev), len(idx), n_total, cap_num, cap_den, max_rounds,
+                                                                        C.byref(m), C.byref(passes)))
+        return m.value, passes.value
+
     def assign_bounded_begin(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
         self._ck(self.L.rio_cuda_set_assign_bounded_begin(self.s, n_total, cap_num, cap_den, max_rounds))
 
