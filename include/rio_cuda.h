@@ -343,7 +343,14 @@ rio_status  rio_cuda_comm_info(rio_placement *h, int32_t *rank, int32_t *world);
 /* all-gather + sum of an M-entry u32 counter vector (host in/out); exposed for tests and host-side logic */
 rio_status  rio_cuda_comm_sum_counters(rio_placement *h, uint32_t *inout, uint32_t M);
 
-/* ---- device-resident variants (inputs already in HBM; asynchronous on the handle's stream) ------------- */
+/* ---- device-resident variants (inputs already in HBM; asynchronous on the handle's stream) -------------
+ * Alignment: every d_ buffer must be naturally aligned for its element type -- 8 bytes for keys, 4 for node indices and
+ * features.  Any other pointer is refused with RIO_ERR_UNKNOWN before anything is enqueued.  Any naturally aligned pointer is
+ * accepted, such as a slice of a larger buffer.  Some kernels take wider loads: the HRW2 walk of assign_batch_dev reads keys 16
+ * bytes and writes indices 8 bytes at a time, and every K == 16 affinity kernel reads feature rows 16 bytes at a time.  When such
+ * a buffer does not start at that alignment, the call copies it on the stream into the handle's own buffer and runs from there;
+ * the copy costs one extra pass over that buffer.  A buffer at 256 bytes, which is what rio_cuda_dev_alloc and cudaMalloc return,
+ * is always used in place.  A call writes exactly n (or n x ranks) entries of d_out_idx and never writes its inputs. */
 rio_status  rio_cuda_dev_alloc(rio_placement *h, size_t bytes, void **out_dev);
 rio_status  rio_cuda_dev_free(rio_placement *h, void *dev);
 rio_status  rio_cuda_host_alloc(rio_placement *h, size_t bytes, void **out_pinned);  /* pinned host memory */

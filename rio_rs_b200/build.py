@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "librio_cuda.so")
 SOURCES = ["k_assign.cu", "k_trie.cu", "k_ranked.cu", "k_spread.cu", "k_affinity_umma.cu", "k_affinity_set.cu", "k_affinity_bounded.cu", "k_set_bounded_affinity.cu", "k_directory.cu", "engine.cu", "resolver.cu", "durable.cu"]
-HEADERS = ["kernels.cuh", "k_ranked.cuh", "k_rank_common.cuh", "k_spread.cuh", "k_affinity_ranked.cuh", "k_affinity_spread.cuh", "k_affinity_set.cuh", "k_affinity_bounded.cuh", "k_set_bounded_affinity.cuh", "k_affinity_common.cuh", "k_changes.cuh", "k_ranked_changes.cuh", "k_spread_changes.cuh", "spec.cuh", "bounded_tail.cuh", "trie_table.hpp", os.path.join("..", "..", "include", "rio_cuda.h"), os.path.join("..", "..", "include", "rio_cuda_dev.h")]
+HEADERS = ["kernels.cuh", "buffer_align.cuh", "k_ranked.cuh", "k_rank_common.cuh", "k_spread.cuh", "k_affinity_ranked.cuh", "k_affinity_spread.cuh", "k_affinity_set.cuh", "k_affinity_bounded.cuh", "k_set_bounded_affinity.cuh", "k_affinity_common.cuh", "k_changes.cuh", "k_ranked_changes.cuh", "k_spread_changes.cuh", "spec.cuh", "bounded_tail.cuh", "trie_table.hpp", os.path.join("..", "..", "include", "rio_cuda.h"), os.path.join("..", "..", "include", "rio_cuda_dev.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

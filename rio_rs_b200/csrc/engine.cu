@@ -784,6 +784,42 @@ void ranked_from_host(rio_placement *h, DevBuf &d_in, const T *in, size_t in_n, 
     CUDA_TRY(cudaStreamSynchronize(st));
 }
 
+// ---- caller buffers of the _dev calls (the alignment rules of buffer_align.cuh) ----------------------------------------------------------
+bool aligned_to(const void *p, uint32_t align) { return ((uintptr_t)p & (align - 1)) == 0; }
+
+// A _dev call refuses a buffer that is not naturally aligned for its element type, before it enqueues anything.
+void require_natural(const void *p, uint32_t align, const char *name) {
+    if (p) REQUIRE(aligned_to(p, align), std::string(name) + " is not aligned to its element size (" + std::to_string(align) + " bytes)");
+}
+
+// A caller's input the launcher reads in place if it starts at `align`; otherwise a copy of it in the handle's staging buffer `buf`,
+// made on the stream.
+template <class T>
+const T *input_at(rio_placement *h, DevBuf &buf, const T *p, size_t count, uint32_t align) {
+    if (aligned_to(p, align)) return p;
+    buf.ensure(count * sizeof(T), h->stream);
+    CUDA_TRY(cudaMemcpyAsync(buf.p, p, count * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
+    return buf.as<const T>();
+}
+
+// Where the launcher writes a caller's output of `count` indices: the buffer itself if it starts at `align`, else the handle's staging
+// buffer `buf`, which output_done then copies into the caller's buffer on the stream.  Staging buffers are reused by the next call
+// only behind that copy, in stream order.
+uint32_t *output_at(rio_placement *h, DevBuf &buf, uint32_t *p, size_t count, uint32_t align) {
+    if (aligned_to(p, align)) return p;
+    buf.ensure(count * 4, h->stream);
+    return buf.as<uint32_t>();
+}
+void output_done(rio_placement *h, const uint32_t *written, uint32_t *p, size_t count) {
+    if (written != p) CUDA_TRY(cudaMemcpyAsync(p, written, count * 4, cudaMemcpyDeviceToDevice, h->stream));
+}
+
+// The feature rows of an affinity _dev call where the launchers of `path` read them; the no-live-node fill reads none.  Every affinity
+// kernel writes its indices one at a time, so the caller's output is used in place.
+const float *affinity_input(rio_placement *h, const float *d_feats, uint64_t n, AffinityPath path) {
+    return path == AffinityPath::kNoLiveNode ? d_feats : input_at(h, h->s_feats, d_feats, n * h->K, affinity_feats_align(h->K));
+}
+
 uint32_t capacity_of(uint64_t n_total, uint32_t w, uint64_t w_sum, uint32_t num, uint32_t den) {
     if (!w || !w_sum || !den) return 0;
     unsigned __int128 a = (unsigned __int128)num * n_total * w, b = (unsigned __int128)den * w_sum;
@@ -1554,12 +1590,23 @@ rio_status rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, c
     return guarded(h, [&] {
         if (!n) return;
         REQUIRE(d_out_idx && (d_keys || d_obj_feats), "null buffer");
-        ensure_tab(h);
+        require_natural(d_keys, 8, "d_keys");
+        require_natural(d_obj_feats, 4, "d_obj_feats");
+        require_natural(d_out_idx, 4, "d_out_idx");
         if (d_obj_feats) {
             REQUIRE(h->K > 0, "assign with object features needs node features");
-            run_affinity(h, d_obj_feats, n, d_out_idx, nullptr, nullptr, affinity_path(h));
+            REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
+            ensure_tab(h);
+            const AffinityPath path = affinity_path(h);
+            run_affinity(h, affinity_input(h, d_obj_feats, n, path), n, d_out_idx, nullptr, nullptr, path);
         } else {
-            run_assign(h, h->solver, h->tabs, d_keys, n, d_out_idx, nullptr, nullptr, 0);
+            ensure_tab(h);
+            // the flat kernels read keys and write indices one at a time; the HRW2 walk two at a time
+            const bool trie = h->solver == RIO_SOLVER_HRW2;
+            const uint64_t *keys = input_at(h, h->s_keys, d_keys, n, trie ? kAlignTrieKeys : 8u);
+            uint32_t *out = output_at(h, h->s_idx, d_out_idx, n, trie ? kAlignTrieOut : 4u);
+            run_assign(h, h->solver, h->tabs, keys, n, out, nullptr, nullptr, 0);
+            output_done(h, out, d_out_idx, n);
         }
     });
 }
@@ -1580,6 +1627,9 @@ rio_status rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(d_keys && d_out_idx, "null buffer");
+        require_natural(d_keys, 8, "d_keys");
+        require_natural(d_out_idx, 4, "d_out_idx");
+        // both ranked walks read keys and write list entries one at a time: the caller's buffers are used in place
         run_assign_ranked(h, d_keys, n, ranks, d_out_idx);
     });
 }
@@ -1600,6 +1650,9 @@ rio_status rio_cuda_assign_ranked_spread_batch_dev(rio_placement *h, const uint6
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(d_keys && d_out_idx, "null buffer");
+        require_natural(d_keys, 8, "d_keys");
+        require_natural(d_out_idx, 4, "d_out_idx");
+        // both failure-domain walks read keys and write list entries one at a time: the caller's buffers are used in place
         run_assign_spread(h, d_keys, n, ranks, d_out_idx);
     });
 }
@@ -1624,9 +1677,13 @@ rio_status rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const flo
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(d_obj_feats && d_out_idx, "null buffer");
+        require_natural(d_obj_feats, 4, "d_obj_feats");
+        require_natural(d_out_idx, 4, "d_out_idx");
         REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
         ensure_tab(h);
-        run_affinity_ranked(h, d_obj_feats, n, ranks, d_out_idx, affinity_path(h));
+        const AffinityPath path = affinity_path(h);
+        run_affinity_ranked(h, affinity_input(h, d_obj_feats, n, path), n, ranks, d_out_idx, path);
     });
 }
 
@@ -1650,15 +1707,25 @@ rio_status rio_cuda_assign_ranked_affinity_spread_batch_dev(rio_placement *h, co
         check_ranked_args(n, ranks);
         if (!n) return;
         REQUIRE(d_obj_feats && d_out_idx, "null buffer");
+        require_natural(d_obj_feats, 4, "d_obj_feats");
+        require_natural(d_out_idx, 4, "d_out_idx");
         REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
         ensure_tab(h);
-        run_affinity_spread(h, d_obj_feats, n, ranks, d_out_idx, affinity_path(h));
+        const AffinityPath path = affinity_path(h);
+        run_affinity_spread(h, affinity_input(h, d_obj_feats, n, path), n, ranks, d_out_idx, path);
     });
 }
 
 rio_status rio_cuda_lookup_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] { if (n) { REQUIRE(d_keys && d_out_idx, "null buffer"); launch_dir_lookup(h->L(), h->dir, d_keys, n, d_out_idx); } });
+    return guarded(h, [&] {
+        if (!n) return;
+        REQUIRE(d_keys && d_out_idx, "null buffer");
+        require_natural(d_keys, 8, "d_keys");
+        require_natural(d_out_idx, 4, "d_out_idx");
+        launch_dir_lookup(h->L(), h->dir, d_keys, n, d_out_idx);   // one key read and one index written at a time: used in place
+    });
 }
 
 rio_status rio_cuda_upsert_batch_dev(rio_placement *h, const uint64_t *d_keys, const uint32_t *d_idx, size_t n) {
@@ -1666,6 +1733,9 @@ rio_status rio_cuda_upsert_batch_dev(rio_placement *h, const uint64_t *d_keys, c
     return guarded(h, [&] {
         if (!n) return;
         REQUIRE(d_keys && d_idx, "null buffer");
+        require_natural(d_keys, 8, "d_keys");
+        require_natural(d_idx, 4, "d_idx");
+        // k_dir_upsert reads one key and one index at a time: the caller's buffers are used in place
         REQUIRE((h->dir_keys + h->dir_keys_pending + n) * 10 <= h->dir_cap * 9, "directory too small for an asynchronous upsert: call rio_cuda_directory_reserve first");
         dir_upsert_dev(h, d_keys, d_idx, 0, n);
         h->dir_keys_pending += n;

@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "buffer_align.cuh"
+
 namespace rio {
 
 // ---- node table as the assign kernels see it -----------------------------------------------------------

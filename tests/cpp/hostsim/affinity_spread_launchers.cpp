@@ -20,6 +20,7 @@ namespace rio {
 void launch_assign_affinity_spread(const Launch &L, const float *fobj, uint64_t n, const float *fnode, const uint32_t *live, uint32_t n_total, uint32_t K,
                                    const uint32_t *ndom, uint32_t ranks, uint32_t *out) {
     if (!n) return;
+    if (hostsim_misaligned(fobj, HOSTSIM_DECLARED_ALIGN(affinity_feats_align(K)))) return;
     std::vector<std::tuple<float, uint32_t>> c;
     std::vector<uint32_t> listed;
     for (uint64_t i = 0; i < n; i++) {

@@ -27,6 +27,7 @@ inline uint2 make_uint2(uint32_t x, uint32_t y) { return uint2{x, y}; }
 typedef int cudaError_t;
 constexpr cudaError_t cudaSuccess = 0;
 constexpr cudaError_t cudaErrorInvalidValue = 1;
+constexpr cudaError_t cudaErrorMisalignedAddress = 716;
 struct HostSimStream { int id; };
 struct HostSimEvent { std::chrono::steady_clock::time_point t; };
 typedef HostSimStream *cudaStream_t;
@@ -38,8 +39,26 @@ constexpr unsigned cudaStreamNonBlocking = 1, cudaEventDisableTiming = 2, cudaHo
 struct cudaDeviceProp { char name[256]; size_t totalGlobalMem; int multiProcessorCount; };
 struct cudaIpcMemHandle_t { char reserved[64]; };
 
-inline const char *cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "host-sim error"; }
-inline cudaError_t cudaGetLastError() { return cudaSuccess; }
+inline const char *cudaGetErrorString(cudaError_t e) {
+    return e == cudaSuccess ? "no error" : e == cudaErrorMisalignedAddress ? "misaligned address" : "host-sim error";
+}
+// The error a launcher double reported, returned (and cleared) by the next cudaGetLastError of the thread, as the runtime does
+inline cudaError_t &hostsim_last_error() { static thread_local cudaError_t e = cudaSuccess; return e; }
+inline cudaError_t cudaGetLastError() { const cudaError_t e = hostsim_last_error(); hostsim_last_error() = cudaSuccess; return e; }
+// The alignment a kernel assumes of a caller's buffer, as csrc/buffer_align.cuh declares it: HOSTSIM_DECLARED_ALIGN(rio::kAlignTrieKeys).
+// Against an engine without that header the doubles check natural alignment only (1 byte: every pointer passes).
+#if __has_include("../../../rio_rs_b200/csrc/buffer_align.cuh")
+#define HOSTSIM_DECLARED_ALIGN(a) (a)
+#else
+#define HOSTSIM_DECLARED_ALIGN(a) 1u
+#endif
+// A launcher double whose kernel reads or writes `p` with loads of `align` bytes calls this first: a pointer the kernel would fault
+// on is reported as the launch error a misaligned access gives (the double then computes nothing), instead of being read silently.
+inline bool hostsim_misaligned(const void *p, size_t align) {
+    if (!p || ((uintptr_t)p & (align - 1)) == 0) return false;
+    hostsim_last_error() = cudaErrorMisalignedAddress;
+    return true;
+}
 inline cudaError_t cudaGetDeviceCount(int *n) { *n = 1; return cudaSuccess; }
 inline cudaError_t cudaGetDevice(int *d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaSetDevice(int) { return cudaSuccess; }
@@ -62,7 +81,8 @@ inline cudaError_t cudaEventRecord(cudaEvent_t e, cudaStream_t) { e->t = std::ch
 inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 inline cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t a, cudaEvent_t b) { *ms = std::chrono::duration<float, std::milli>(b->t - a->t).count(); return cudaSuccess; }
 inline cudaError_t cudaEventDestroy(cudaEvent_t e) { delete e; return cudaSuccess; }
-inline cudaError_t cudaMalloc(void **p, size_t n) { *p = malloc(n ? n : 1); return *p ? cudaSuccess : cudaErrorInvalidValue; }
+// 256-byte aligned, as device allocations are (glibc's malloc gives 16)
+inline cudaError_t cudaMalloc(void **p, size_t n) { *p = aligned_alloc(256, ((n ? n : 1) + 255) / 256 * 256); return *p ? cudaSuccess : cudaErrorInvalidValue; }
 inline cudaError_t cudaFree(void *p) { free(p); return cudaSuccess; }
 inline cudaError_t cudaMallocAsync(void **p, size_t n, cudaStream_t) { return cudaMalloc(p, n); }
 inline cudaError_t cudaFreeAsync(void *p, cudaStream_t) { return cudaFree(p); }

@@ -118,6 +118,7 @@ void launch_assign_trie(const Launch &L, const uint64_t *keys, uint64_t n, const
                         const BoundedTail *tail) {
     const uint64_t n_work = sel ? n_sel : n;
     if (!n_work) return;
+    if (!sel && (hostsim_misaligned(keys, HOSTSIM_DECLARED_ALIGN(kAlignTrieKeys)) || hostsim_misaligned(out, HOSTSIM_DECLARED_ALIGN(kAlignTrieOut)))) return;   // the dense walk's vector accesses
     for (uint64_t q = 0; q < n_work; q++) {
         const uint64_t i = sel ? sel[q] : q;
         const uint32_t j = walk(keys[i], t);
@@ -152,6 +153,7 @@ void launch_dir_reassign_trie(const Launch &L, const DirDev &dir, const TrieDev 
 void launch_assign_affinity(const Launch &L, const float *fobj, uint64_t n, const float *fnode, const uint32_t *live, uint32_t n_total, uint32_t K, uint32_t *out, float *out_cost,
                             uint32_t *counters) {
     if (!n) return;
+    if (hostsim_misaligned(fobj, HOSTSIM_DECLARED_ALIGN(affinity_feats_align(K)))) return;
     for (uint64_t i = 0; i < n; i++) {
         float best = 0.f;
         uint32_t bj = kNone;
