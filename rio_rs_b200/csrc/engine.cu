@@ -159,6 +159,13 @@ struct BoundedState {
     void release(cudaStream_t st) { buf.release(st); if (h_flags) cudaFreeHost(h_flags); h_flags = nullptr; if (ev) cudaEventDestroy(ev); ev = nullptr; }
 };
 
+// The kind of a ranked call's or a resident set's lists, from keys: each object's first R nodes under the handle's policy (kHash,
+// DESIGN.md 3.9) or its first R nodes in R distinct failure domains (kSpread, 3.12); from feature rows: its R lowest-cost nodes
+// (kAffinity, 3.9) or those in R distinct domains (kAffinitySpread, 3.14)
+enum class ListKind { kHash, kSpread, kAffinity, kAffinitySpread };
+bool is_affinity(ListKind k) { return k == ListKind::kAffinity || k == ListKind::kAffinitySpread; }
+bool is_spread(ListKind k) { return k == ListKind::kSpread || k == ListKind::kAffinitySpread; }
+
 }  // namespace
 
 struct rio_placement {
@@ -246,25 +253,25 @@ struct rio_objset {
     BoundedState bs;
     bool assigned = false;
     // ranked lists (DESIGN.md 3.11): n x ranks row-major, column 0 == idx; ranks == 0 = the set holds none.  The buffer is grow-only
-    // (capacity x ranks), the lists record the policy they were computed under.
+    // (capacity x ranks), the lists record their kind (meaningful while ranks != 0) and the policy they were computed under.
     DevBuf lists;
     uint32_t ranks = 0, rank_solver = 0, rank_bits = 0;
-    // spread lists (DESIGN.md 3.13): the lists are failure-domain lists, computed under the labels of label_snap (one per node interned
+    ListKind kind = ListKind::kHash;
+    // spread kinds (DESIGN.md 3.13): the lists are failure-domain lists, computed under the labels of label_snap (one per node interned
     // then; a node interned later had RIO_NONE), which were the handle's labels at label_version label_snap_version
-    bool spread = false;
     std::vector<uint32_t> label_snap;
     uint64_t label_snap_version = 0;
-    // affinity lists (DESIGN.md 3.15): the lists are affinity lists of the set's features (spread says which kind), computed on the
-    // tensor cores (aff_tensor) or the CUDA cores under the handle's K aff_K, with the node features of feat_snap (aff_K floats per node
-    // interned then; a row that was not K wide is zeros, as the kernels see it), the handle's at feat_version feat_snap_version
-    bool affinity = false, aff_tensor = false;
+    // affinity kinds (DESIGN.md 3.15): the lists are affinity lists of the set's features, computed on the tensor cores (aff_tensor) or
+    // the CUDA cores under the handle's K aff_K, with the node features of feat_snap (aff_K floats per node interned then; a row that
+    // was not K wide is zeros, as the kernels see it), the handle's at feat_version feat_snap_version
+    bool aff_tensor = false;
     uint32_t aff_K = 0;
     std::vector<float> feat_snap;
     uint64_t feat_snap_version = 0;
     // bounded-load affinity record (DESIGN.md 3.17): idx is the result of set_assign_bounded_affinity or of the change-set call that
     // keeps it, on the path of aff_tensor under aff_K, with the node features of feat_snap.  Cleared with the lists and by load_feats.
     bool bounded_aff = false;
-    void drop_lists() { ranks = 0; spread = false; affinity = false; bounded_aff = false; }
+    void drop_lists() { ranks = 0; kind = ListKind::kHash; bounded_aff = false; }
 };
 
 namespace {
@@ -587,19 +594,6 @@ void check_ranked_args(size_t n, uint32_t ranks) {
     REQUIRE(n <= SIZE_MAX / 4 / ranks, "n x ranks overflows");
 }
 
-// each object's first `ranks` distinct nodes under the handle's policy (DESIGN.md 3.9)
-void run_assign_ranked(rio_placement *h, const uint64_t *d_keys, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
-    if (!launch_assign_hrw_ranked || !launch_assign_trie_ranked)
-        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked kernels (k_ranked.cu is not linked)"};
-    ensure_tab(h);
-    if (h->solver == RIO_SOLVER_HRW2) {
-        ensure_rank_tab(h);
-        launch_assign_trie_ranked(h->L(), d_keys, n, h->tabs.trie, h->rank_tab, ranks, d_out_idx);
-    } else {
-        launch_assign_hrw_ranked(h->L(), d_keys, n, h->tabs.tab, ranks, d_out_idx);
-    }
-}
-
 // Dense domain ids of the live nodes per interned index (kNone for the others): one per label shared by live nodes, one per live
 // node labelled RIO_NONE, numbered in node-index order.  Returns the number of domains.
 uint32_t dense_domains(const rio_placement *h, std::vector<uint32_t> &ndom) {
@@ -676,16 +670,6 @@ void ensure_spread_tab(rio_placement *h) {
     h->spread_version[1] = h->label_version;
 }
 
-// each object's first `ranks` nodes in distinct failure domains under the handle's policy (DESIGN.md 3.12)
-void run_assign_spread(rio_placement *h, const uint64_t *d_keys, uint64_t n, uint32_t ranks, uint32_t *d_out_idx) {
-    if (!launch_assign_hrw_spread || !launch_assign_trie_spread)
-        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no spread kernels (k_spread.cu is not linked)"};
-    ensure_tab(h);
-    ensure_spread_tab(h);
-    if (h->solver == RIO_SOLVER_HRW2) launch_assign_trie_spread(h->L(), d_keys, n, h->tabs.trie, h->spread_tab, ranks, d_out_idx);
-    else launch_assign_hrw_spread(h->L(), d_keys, n, h->tabs.tab, h->spread_tab, ranks, d_out_idx);
-}
-
 // affinity dispatch: no live node fills the output with NONE; the tensor-core (wgmma) kernel for K == 16 (unless
 // RIO_AFFINITY_VARIANT=ffma or the node set does not fit); else the CUDA cores
 enum class AffinityPath { kNoLiveNode, kTensorCores, kCudaCores };
@@ -714,24 +698,6 @@ void run_affinity(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t *d
     }
 }
 
-// each object's `ranks` lowest-cost live nodes (DESIGN.md 3.9), on the path run_affinity takes for the same handle and environment,
-// so that rank 1 is its answer, or on `path`; the tensor-core pair keeps its per-object groups in s_idx2 between the two passes
-void run_affinity_ranked(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx, AffinityPath path) {
-    if (!launch_assign_affinity_ranked || !launch_assign_affinity_umma_ranked)
-        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked affinity kernels (k_affinity_umma.cu / k_assign.cu are not linked)"};
-    switch (path) {
-        case AffinityPath::kNoLiveNode: launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); break;
-        case AffinityPath::kTensorCores:
-            h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
-            CUDA_TRY(launch_assign_affinity_umma_ranked(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
-                                                        h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
-            break;
-        case AffinityPath::kCudaCores:
-            launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
-            break;
-    }
-}
-
 // The domain ids of the failure-domain affinity lists: without the HRW2 blob ensure_spread_tab builds, so the first call after a
 // relabel costs one pass over the nodes and one small copy
 void ensure_aff_dom(rio_placement *h) {
@@ -754,34 +720,60 @@ void ensure_aff_dom(rio_placement *h) {
     h->aff_dom_version[1] = h->label_version;
 }
 
-// each object's `ranks` lowest-cost live nodes in distinct failure domains (DESIGN.md 3.14), on the path run_affinity takes, so that
-// rank 1 is its answer, or on `path`; the tensor-core pair keeps each object's listed column positions in s_idx2 between the two passes
-void run_affinity_spread(rio_placement *h, const float *d_fobj, uint64_t n, uint32_t ranks, uint32_t *d_out_idx, AffinityPath path) {
-    if (!launch_assign_affinity_spread || !launch_assign_affinity_umma_spread)
-        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no failure-domain affinity kernels (k_affinity_spread.cuh launchers are not linked)"};
+// The n x ranks lists of `kind` (see ListKind) for the n keys or feature rows at `in` into d_out_idx, under the handle's policy.  The
+// affinity kinds run on `path` (the batch calls pass affinity_path(h), so that rank 1 is run_affinity's answer; a resident set passes
+// its recorded path), and their tensor-core pairs keep each object's groups or listed column positions in s_idx2 between the two
+// passes.  A build without the kind's kernels refuses before anything is launched.
+void run_lists(rio_placement *h, ListKind kind, const void *in, uint64_t n, uint32_t ranks, uint32_t *d_out_idx, AffinityPath path) {
+    const uint64_t *d_keys = static_cast<const uint64_t *>(in);
+    switch (kind) {
+        case ListKind::kHash:
+            if (!launch_assign_hrw_ranked || !launch_assign_trie_ranked)
+                throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked kernels (k_ranked.cu is not linked)"};
+            ensure_tab(h);
+            if (h->solver == RIO_SOLVER_HRW2) {
+                ensure_rank_tab(h);
+                launch_assign_trie_ranked(h->L(), d_keys, n, h->tabs.trie, h->rank_tab, ranks, d_out_idx);
+            } else {
+                launch_assign_hrw_ranked(h->L(), d_keys, n, h->tabs.tab, ranks, d_out_idx);
+            }
+            return;
+        case ListKind::kSpread:
+            if (!launch_assign_hrw_spread || !launch_assign_trie_spread)
+                throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no spread kernels (k_spread.cu is not linked)"};
+            ensure_tab(h);
+            ensure_spread_tab(h);
+            if (h->solver == RIO_SOLVER_HRW2) launch_assign_trie_spread(h->L(), d_keys, n, h->tabs.trie, h->spread_tab, ranks, d_out_idx);
+            else launch_assign_hrw_spread(h->L(), d_keys, n, h->tabs.tab, h->spread_tab, ranks, d_out_idx);
+            return;
+        case ListKind::kAffinity:
+            if (!launch_assign_affinity_ranked || !launch_assign_affinity_umma_ranked)
+                throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked affinity kernels (k_affinity_umma.cu / k_assign.cu are not linked)"};
+            break;
+        case ListKind::kAffinitySpread:
+            if (!launch_assign_affinity_spread || !launch_assign_affinity_umma_spread)
+                throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no failure-domain affinity kernels (k_affinity_spread.cuh launchers are not linked)"};
+            break;
+    }
+    if (!n) return;   // an empty resident set: no list to compute, no domain table needed
+    const float *d_fobj = static_cast<const float *>(in);
+    const bool spread = kind == ListKind::kAffinitySpread;
     if (path == AffinityPath::kNoLiveNode) { launch_fill_u32(h->L(), d_out_idx, n * ranks, kNone); return; }
-    ensure_aff_dom(h);
+    if (spread) ensure_aff_dom(h);
     const uint32_t *ndom = h->aff_dom.as<uint32_t>();
     if (path == AffinityPath::kTensorCores) {
         h->s_idx2.ensure(n * affinity_ranked_groups(ranks) * 4, h->stream);
-        CUDA_TRY(launch_assign_affinity_umma_spread(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
-                                                    ndom + h->aff_dom_pos, h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
-    } else {
+        if (spread)
+            CUDA_TRY(launch_assign_affinity_umma_spread(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
+                                                        ndom + h->aff_dom_pos, h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
+        else
+            CUDA_TRY(launch_assign_affinity_umma_ranked(h->L(), d_fobj, n, h->d_fnode_c.as<float>(), h->d_fnode_g.as<float>(), h->d_nidx_map.as<uint32_t>(),
+                                                        h->aff_live, h->aff_pad, ranks, h->s_idx2.as<uint32_t>(), d_out_idx));
+    } else if (spread) {
         launch_assign_affinity_spread(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ndom, ranks, d_out_idx);
+    } else {
+        launch_assign_affinity_ranked(h->L(), d_fobj, n, h->d_fnode.as<float>(), h->tabs.live, h->tabs.tab.n_total, h->K, ranks, d_out_idx);
     }
-}
-
-// The host-buffer form of a ranked call: in_n elements from `in` into d_in, run(d_in, h->s_idx) on the device, the n x ranks lists
-// back into out_idx, and the stream synchronised
-template <class T, class F>
-void ranked_from_host(rio_placement *h, DevBuf &d_in, const T *in, size_t in_n, size_t n, uint32_t ranks, uint32_t *out_idx, F &&run) {
-    cudaStream_t st = h->stream;
-    d_in.ensure(in_n * sizeof(T), st);
-    h->s_idx.ensure(n * ranks * 4, st);
-    CUDA_TRY(cudaMemcpyAsync(d_in.p, in, in_n * sizeof(T), cudaMemcpyHostToDevice, st));
-    run(d_in.as<const T>(), h->s_idx.as<uint32_t>());
-    CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
 }
 
 // ---- caller buffers of the _dev calls (the alignment rules of buffer_align.cuh) ----------------------------------------------------------
@@ -818,6 +810,47 @@ void output_done(rio_placement *h, const uint32_t *written, uint32_t *p, size_t 
 // kernel writes its indices one at a time, so the caller's output is used in place.
 const float *affinity_input(rio_placement *h, const float *d_feats, uint64_t n, AffinityPath path) {
     return path == AffinityPath::kNoLiveNode ? d_feats : input_at(h, h->s_feats, d_feats, n * h->K, affinity_feats_align(h->K));
+}
+
+// The path of an affinity list batch of n rows, once the handle's K admits it, with the table current; the hash kinds take none
+AffinityPath list_batch_path(rio_placement *h, ListKind kind, size_t n) {
+    if (!is_affinity(kind)) return AffinityPath::kCudaCores;
+    REQUIRE(h->K > 0, "assign with object features needs node features");
+    REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
+    ensure_tab(h);
+    return affinity_path(h);
+}
+
+// The host-buffer form of a list call: keys staged through s_keys or feature rows through s_feats, the n x ranks lists through s_idx
+// back into out_idx, and the stream synchronised
+void lists_from_host(rio_placement *h, ListKind kind, const void *in, size_t n, uint32_t ranks, uint32_t *out_idx) {
+    check_ranked_args(n, ranks);
+    if (!n) return;
+    REQUIRE(in && out_idx, "null buffer");
+    const AffinityPath path = list_batch_path(h, kind, n);
+    DevBuf &d_in = is_affinity(kind) ? h->s_feats : h->s_keys;
+    const size_t in_bytes = is_affinity(kind) ? n * h->K * 4 : n * 8;
+    cudaStream_t st = h->stream;
+    d_in.ensure(in_bytes, st);
+    h->s_idx.ensure(n * ranks * 4, st);
+    CUDA_TRY(cudaMemcpyAsync(d_in.p, in, in_bytes, cudaMemcpyHostToDevice, st));
+    run_lists(h, kind, d_in.p, n, ranks, h->s_idx.as<uint32_t>(), path);
+    CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * ranks * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+}
+
+// The device-buffer form: every list kernel reads keys and writes list entries one at a time, so those buffers are used in place;
+// feature rows are read where affinity_input puts them
+void lists_from_device(rio_placement *h, ListKind kind, const void *d_in, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
+    check_ranked_args(n, ranks);
+    if (!n) return;
+    REQUIRE(d_in && d_out_idx, "null buffer");
+    if (is_affinity(kind)) require_natural(d_in, 4, "d_obj_feats");
+    else require_natural(d_in, 8, "d_keys");
+    require_natural(d_out_idx, 4, "d_out_idx");
+    const AffinityPath path = list_batch_path(h, kind, n);
+    if (is_affinity(kind)) d_in = affinity_input(h, static_cast<const float *>(d_in), n, path);
+    run_lists(h, kind, d_in, n, ranks, d_out_idx, path);
 }
 
 uint32_t capacity_of(uint64_t n_total, uint32_t w, uint64_t w_sum, uint32_t num, uint32_t den) {
@@ -1613,108 +1646,42 @@ rio_status rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, c
 
 rio_status rio_cuda_assign_ranked_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(keys && out_idx, "null buffer");
-        ranked_from_host(h, h->s_keys, keys, n, n, ranks, out_idx, [&](const uint64_t *d_keys, uint32_t *d_out) { run_assign_ranked(h, d_keys, n, ranks, d_out); });
-    });
+    return guarded(h, [&] { lists_from_host(h, ListKind::kHash, keys, n, ranks, out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(d_keys && d_out_idx, "null buffer");
-        require_natural(d_keys, 8, "d_keys");
-        require_natural(d_out_idx, 4, "d_out_idx");
-        // both ranked walks read keys and write list entries one at a time: the caller's buffers are used in place
-        run_assign_ranked(h, d_keys, n, ranks, d_out_idx);
-    });
+    return guarded(h, [&] { lists_from_device(h, ListKind::kHash, d_keys, n, ranks, d_out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_spread_batch(rio_placement *h, const uint64_t *keys, size_t n, uint32_t ranks, uint32_t *out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(keys && out_idx, "null buffer");
-        ranked_from_host(h, h->s_keys, keys, n, n, ranks, out_idx, [&](const uint64_t *d_keys, uint32_t *d_out) { run_assign_spread(h, d_keys, n, ranks, d_out); });
-    });
+    return guarded(h, [&] { lists_from_host(h, ListKind::kSpread, keys, n, ranks, out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_spread_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(d_keys && d_out_idx, "null buffer");
-        require_natural(d_keys, 8, "d_keys");
-        require_natural(d_out_idx, 4, "d_out_idx");
-        // both failure-domain walks read keys and write list entries one at a time: the caller's buffers are used in place
-        run_assign_spread(h, d_keys, n, ranks, d_out_idx);
-    });
+    return guarded(h, [&] { lists_from_device(h, ListKind::kSpread, d_keys, n, ranks, d_out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_affinity_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(obj_feats && out_idx, "null buffer");
-        REQUIRE(h->K > 0, "assign with object features needs node features");
-        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
-        ensure_tab(h);
-        ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
-                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_ranked(h, d_feats, n, ranks, d_out, affinity_path(h)); });
-    });
+    return guarded(h, [&] { lists_from_host(h, ListKind::kAffinity, obj_feats, n, ranks, out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_affinity_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(d_obj_feats && d_out_idx, "null buffer");
-        require_natural(d_obj_feats, 4, "d_obj_feats");
-        require_natural(d_out_idx, 4, "d_out_idx");
-        REQUIRE(h->K > 0, "assign with object features needs node features");
-        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
-        ensure_tab(h);
-        const AffinityPath path = affinity_path(h);
-        run_affinity_ranked(h, affinity_input(h, d_obj_feats, n, path), n, ranks, d_out_idx, path);
-    });
+    return guarded(h, [&] { lists_from_device(h, ListKind::kAffinity, d_obj_feats, n, ranks, d_out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_affinity_spread_batch(rio_placement *h, const float *obj_feats, size_t n, uint32_t ranks, uint32_t *out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(obj_feats && out_idx, "null buffer");
-        REQUIRE(h->K > 0, "assign with object features needs node features");
-        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
-        ensure_tab(h);
-        ranked_from_host(h, h->s_feats, obj_feats, n * h->K, n, ranks, out_idx,
-                         [&](const float *d_feats, uint32_t *d_out) { run_affinity_spread(h, d_feats, n, ranks, d_out, affinity_path(h)); });
-    });
+    return guarded(h, [&] { lists_from_host(h, ListKind::kAffinitySpread, obj_feats, n, ranks, out_idx); });
 }
 
 rio_status rio_cuda_assign_ranked_affinity_spread_batch_dev(rio_placement *h, const float *d_obj_feats, size_t n, uint32_t ranks, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
-    return guarded(h, [&] {
-        check_ranked_args(n, ranks);
-        if (!n) return;
-        REQUIRE(d_obj_feats && d_out_idx, "null buffer");
-        require_natural(d_obj_feats, 4, "d_obj_feats");
-        require_natural(d_out_idx, 4, "d_out_idx");
-        REQUIRE(h->K > 0, "assign with object features needs node features");
-        REQUIRE(n <= SIZE_MAX / 4 / h->K, "n x K overflows");
-        ensure_tab(h);
-        const AffinityPath path = affinity_path(h);
-        run_affinity_spread(h, affinity_input(h, d_obj_feats, n, path), n, ranks, d_out_idx, path);
-    });
+    return guarded(h, [&] { lists_from_device(h, ListKind::kAffinitySpread, d_obj_feats, n, ranks, d_out_idx); });
 }
 
 rio_status rio_cuda_lookup_batch_dev(rio_placement *h, const uint64_t *d_keys, size_t n, uint32_t *d_out_idx) {
@@ -1867,6 +1834,22 @@ namespace {
 struct ChangeSetHost {
     std::vector<uint8_t> bytes;   // n_total flag bytes, padded to 4, then the candidate indices
     uint32_t n_cand = 0;
+    // every interned node not live now is REPLACE; the caller's rule classifies the changed live nodes with mark()
+    explicit ChangeSetHost(const rio_placement *h) {
+        const uint32_t n_total = (uint32_t)h->nodes.size();
+        bytes.assign(std::max<size_t>((n_total + 3) & ~(size_t)3, 4), 0);
+        for (uint32_t j = 0; j < n_total; j++) if (!h->nodes[j].live()) bytes[j] = kChgReplace;
+    }
+    // node j's flags become `flags`; a CANDIDATE goes onto the candidate list once
+    void mark(uint32_t j, uint8_t flags) {
+        if ((flags & kChgCandidate) && !(bytes[j] & kChgCandidate)) {
+            const size_t o = bytes.size();
+            bytes.resize(o + 4);
+            memcpy(bytes.data() + o, &j, 4);
+            n_cand++;
+        }
+        bytes[j] = flags;
+    }
 };
 
 void check_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
@@ -1881,38 +1864,21 @@ void check_change_set(const rio_placement *h, const uint32_t *idx, const uint32_
 }
 
 ChangeSetHost build_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
-    const uint32_t n_total = (uint32_t)h->nodes.size();
-    const size_t pad = (n_total + 3) & ~(size_t)3;
-    ChangeSetHost cs;
-    cs.bytes.assign(std::max<size_t>(pad, 4), 0);
-    for (uint32_t j = 0; j < n_total; j++) if (!h->nodes[j].live()) cs.bytes[j] = kChgReplace;
-    std::vector<uint32_t> cand;
+    ChangeSetHost cs(h);
     for (size_t i = 0; i < k; i++) {
         const NodeInfo &ni = h->nodes[idx[i]];
         if (!ni.live()) continue;   // REPLACE already
         const uint32_t r_prev = prev_weight[i] ? inv_weight(prev_weight[i]) : 0u, r_now = inv_weight(ni.weight);
-        if (r_prev && r_now > r_prev) cs.bytes[idx[i]] = kChgReplace;                     // lost weight
-        else if (!r_prev || r_now < r_prev) { cs.bytes[idx[i]] = kChgCandidate; cand.push_back(idx[i]); }   // joined or gained weight
+        if (r_prev && r_now > r_prev) cs.mark(idx[i], kChgReplace);                  // lost weight
+        else if (!r_prev || r_now < r_prev) cs.mark(idx[i], kChgCandidate);          // joined or gained weight
     }
-    cs.n_cand = (uint32_t)cand.size();
-    const size_t o = cs.bytes.size();
-    cs.bytes.resize(o + cand.size() * 4);
-    if (!cand.empty()) memcpy(cs.bytes.data() + o, cand.data(), cand.size() * 4);
     return cs;
 }
 
 // Spread lists (DESIGN.md 3.13): a relabelled live node is REPLACE | CANDIDATE.  Lists holding it are recomputed; every other list
 // considers it under its new label.
 void add_relabels(ChangeSetHost &cs, const std::vector<uint32_t> &relabelled) {
-    for (uint32_t j : relabelled) {
-        if (!(cs.bytes[j] & kChgCandidate)) {
-            const size_t o = cs.bytes.size();
-            cs.bytes.resize(o + 4);
-            memcpy(cs.bytes.data() + o, &j, 4);
-            cs.n_cand++;
-        }
-        cs.bytes[j] = kChgReplace | kChgCandidate;
-    }
+    for (uint32_t j : relabelled) cs.mark(j, kChgReplace | kChgCandidate);
 }
 
 ChangeSetDev upload_change_set(rio_placement *h, const ChangeSetHost &cs) {
@@ -2025,7 +1991,7 @@ rio_status rio_cuda_set_load_feats(rio_objset *s, const float *feats, uint32_t K
         s->feats.ensure(s->n * (size_t)K * 4, h->stream);
         CUDA_TRY(cudaMemcpyAsync(s->feats.p, feats, s->n * (size_t)K * 4, cudaMemcpyHostToDevice, h->stream));
         s->K = K;
-        if (s->affinity) s->drop_lists();   // affinity lists are lists of the features just replaced; hash lists stay
+        if (is_affinity(s->kind)) s->drop_lists();   // affinity lists are lists of the features just replaced; hash lists stay
         s->bounded_aff = false;
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
@@ -2229,29 +2195,6 @@ std::vector<uint32_t> relabelled_live(const rio_objset *s) {
     return out;
 }
 
-// set_assign_ranked (3.11) and set_assign_ranked_spread (3.13): fresh lists, column 0 into idx, the counters rebuilt from it, and the
-// policy (and for spread lists the labels) they were computed under recorded
-void set_assign_lists(rio_objset *s, uint32_t ranks, bool spread) {
-    rio_placement *h = s->h;
-    check_ranked_args(s->n, ranks);
-    if (spread) require_spread_set_kernels(h->solver);
-    else require_ranked_set_kernels(h->solver);
-    s->drop_lists();
-    s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
-    set_ensure_counters(s);
-    if (spread) run_assign_spread(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
-    else run_assign_ranked(h, s->keys.as<uint64_t>(), s->n, ranks, s->lists.as<uint32_t>());
-    launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
-    set_zero_counters(s);
-    launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
-    s->assigned = true;
-    s->ranks = ranks;
-    s->rank_solver = h->solver;
-    s->rank_bits = h->trie_bits;
-    s->spread = spread;
-    if (spread) snapshot_labels(s);
-}
-
 // ---- affinity resident sets (DESIGN.md 3.15) ------------------------------------------------------------------------------------
 void require_affinity_set_kernels(bool spread) {
     const bool have = launch_ranked_primary && launch_scatter_ranked && launch_rebalance_changes_affinity && launch_gather_rows &&
@@ -2300,38 +2243,37 @@ std::vector<uint32_t> refeatured_live(const rio_objset *s) {
 // live now and CANDIDATES every changed node live now that was not live before; a live -> live weight change is a no-op.  The
 // refeatured (and, for failure-domain lists, relabelled) live nodes are added as REPLACE | CANDIDATE by the caller.
 ChangeSetHost build_affinity_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
-    const uint32_t n_total = (uint32_t)h->nodes.size();
-    const size_t pad = (n_total + 3) & ~(size_t)3;
-    ChangeSetHost cs;
-    cs.bytes.assign(std::max<size_t>(pad, 4), 0);
-    for (uint32_t j = 0; j < n_total; j++) if (!h->nodes[j].live()) cs.bytes[j] = kChgReplace;
-    std::vector<uint32_t> cand;
+    ChangeSetHost cs(h);
     for (size_t i = 0; i < k; i++)
-        if (h->nodes[idx[i]].live() && !prev_weight[i]) { cs.bytes[idx[i]] = kChgCandidate; cand.push_back(idx[i]); }
-    cs.n_cand = (uint32_t)cand.size();
-    const size_t o = cs.bytes.size();
-    cs.bytes.resize(o + cand.size() * 4);
-    if (!cand.empty()) memcpy(cs.bytes.data() + o, cand.data(), cand.size() * 4);
+        if (h->nodes[idx[i]].live() && !prev_weight[i]) cs.mark(idx[i], kChgCandidate);
     return cs;
 }
 
-// set_assign_ranked_affinity(_spread): fresh lists of the set's features on the path affinity_path() gives now, column 0 into idx,
-// the counters rebuilt from it, and the kind, path, K, node features (and labels) they were computed under recorded
-void set_assign_affinity_lists(rio_objset *s, uint32_t ranks, bool spread) {
+// the kernels a resident set of `kind` needs (the hash kinds' depend on the handle's solver)
+void require_set_kernels(ListKind kind, uint32_t solver) {
+    if (is_affinity(kind)) require_affinity_set_kernels(is_spread(kind));
+    else if (is_spread(kind)) require_spread_set_kernels(solver);
+    else require_ranked_set_kernels(solver);
+}
+
+// set_assign_ranked (3.11), set_assign_ranked_spread (3.13) and set_assign_ranked_affinity(_spread) (3.15): fresh lists of `kind`, the
+// affinity kinds on the path affinity_path() gives now, column 0 into idx, the counters rebuilt from it, and what the lists were
+// computed under recorded: the policy, for the affinity kinds the path, K and node features, for the spread kinds the labels
+void set_assign_lists(rio_objset *s, ListKind kind, uint32_t ranks) {
     rio_placement *h = s->h;
+    const bool affinity = is_affinity(kind);
     check_ranked_args(s->n, ranks);
-    REQUIRE(h->K > 0, "assign with object features needs node features");
-    REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
-    require_affinity_set_kernels(spread);
+    if (affinity) {
+        REQUIRE(h->K > 0, "assign with object features needs node features");
+        REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+    }
+    require_set_kernels(kind, h->solver);
     ensure_tab(h);
     s->drop_lists();
     s->lists.ensure(std::max<uint64_t>(s->capacity, 1) * ranks * 4, h->stream);
     set_ensure_counters(s);
     const AffinityPath path = affinity_path(h);
-    if (s->n) {
-        if (spread) run_affinity_spread(h, s->feats.as<float>(), s->n, ranks, s->lists.as<uint32_t>(), path);
-        else run_affinity_ranked(h, s->feats.as<float>(), s->n, ranks, s->lists.as<uint32_t>(), path);
-    }
+    run_lists(h, kind, affinity ? s->feats.p : s->keys.p, s->n, ranks, s->lists.as<uint32_t>(), path);
     launch_ranked_primary(h->L(), s->lists.as<uint32_t>(), s->n, ranks, s->idx.as<uint32_t>());
     set_zero_counters(s);
     launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), s->counters_n);
@@ -2339,51 +2281,74 @@ void set_assign_affinity_lists(rio_objset *s, uint32_t ranks, bool spread) {
     s->ranks = ranks;
     s->rank_solver = h->solver;
     s->rank_bits = h->trie_bits;
-    s->spread = spread;
-    s->affinity = true;
-    record_affinity(s, path);
-    if (spread) snapshot_labels(s);
+    s->kind = kind;
+    if (affinity) record_affinity(s, path);
+    if (is_spread(kind)) snapshot_labels(s);
 }
 
-// set_rebalance_changes_ranked on affinity lists (DESIGN.md 3.15): one pass classifies every list (S1 to s->sel, S2 rows merged with
-// the candidates in place), then the S1 rows are recomputed on the recorded path and scattered back
-void rebalance_affinity_lists(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t &moved, uint64_t &changed) {
+// set_rebalance_changes_ranked (DESIGN.md 3.11, 3.13, 3.15): one pass classifies every list (S1 to s->sel, S2 rows merged with the
+// candidates in place), then the S1 rows are computed afresh and scattered back; hash lists under HRW2 re-walk every key instead.
+// The relabels (spread kinds) and refeatures (affinity kinds) since the set's snapshots belong to the change set.
+void rebalance_lists(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t &moved, uint64_t &changed) {
     rio_placement *h = s->h;
-    const bool spread = s->spread;
-    const uint32_t R = s->ranks, K = s->aff_K;
-    const std::vector<uint32_t> refeatured = refeatured_live(s);
+    const ListKind kind = s->kind;
+    const bool affinity = is_affinity(kind), spread = is_spread(kind);
+    const uint32_t R = s->ranks;
+    const std::vector<uint32_t> refeatured = affinity ? refeatured_live(s) : std::vector<uint32_t>{};
     const std::vector<uint32_t> relabelled = spread ? relabelled_live(s) : std::vector<uint32_t>{};
     if (k || !refeatured.empty() || !relabelled.empty()) {
         ensure_tab(h);
-        if (spread) ensure_aff_dom(h);
+        if (kind == ListKind::kSpread) ensure_spread_tab(h);
+        if (kind == ListKind::kAffinitySpread) ensure_aff_dom(h);
         set_ensure_counters(s);
         zero_scalar(h, S_MOVED);
         zero_scalar(h, S_CHANGED);
-        zero_scalar(h, S_NSEL);
-        ChangeSetHost cs = build_affinity_change_set(h, idx, prev_weight, k);
-        add_relabels(cs, refeatured);
-        add_relabels(cs, relabelled);
-        const ChangeSetDev dcs = upload_change_set(h, cs);
-        uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>();
+        uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>(), *sel = s->sel.as<uint32_t>();
+        const uint64_t *keys = s->keys.as<uint64_t>();
         const uint32_t n_total = h->tabs.tab.n_total;
-        launch_rebalance_changes_affinity(h->L(), s->feats.as<float>(), K, lists, R, d_idx, s->n, h->d_fnode.as<float>(), n_total, dcs,
-                                          spread ? h->aff_dom.as<uint32_t>() : nullptr, counters, s->sel.as<uint32_t>(), h->d_scalars + S_NSEL,
-                                          h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-        const uint64_t n_sel = read_scalar(h, S_NSEL);
-        if (n_sel) {   // S1: the selected objects' lists computed afresh on the recorded path, scattered back
-            h->s_feats.ensure(n_sel * K * 4, h->stream);
-            h->s_idx.ensure(n_sel * R * 4, h->stream);
-            launch_gather_rows(h->L(), s->feats.as<float>(), K, s->sel.as<uint32_t>(), n_sel, h->s_feats.as<float>());
-            const AffinityPath path = affinity_path(h, s->aff_tensor);
-            if (spread) run_affinity_spread(h, h->s_feats.as<float>(), n_sel, R, h->s_idx.as<uint32_t>(), path);
-            else run_affinity_ranked(h, h->s_feats.as<float>(), n_sel, R, h->s_idx.as<uint32_t>(), path);
-            launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel, R, lists, d_idx, counters, n_total, h->d_scalars + S_MOVED,
-                                  h->d_scalars + S_CHANGED);
+        unsigned long long *d_nsel = h->d_scalars + S_NSEL, *d_moved = h->d_scalars + S_MOVED, *d_changed = h->d_scalars + S_CHANGED;
+        if (!affinity && h->solver == RIO_SOLVER_HRW2) {   // one ranked re-walk of every key, only the changed rows written
+            if (spread) {
+                launch_reassign_trie_spread(h->L(), keys, s->n, h->tabs.trie, h->spread_tab, R, lists, d_idx, counters, n_total, d_moved, d_changed);
+            } else {
+                ensure_rank_tab(h);
+                launch_reassign_trie_ranked(h->L(), keys, s->n, h->tabs.trie, h->rank_tab, R, lists, d_idx, counters, n_total, d_moved, d_changed);
+            }
+        } else {
+            ChangeSetHost cs = affinity ? build_affinity_change_set(h, idx, prev_weight, k) : build_change_set(h, idx, prev_weight, k);
+            add_relabels(cs, refeatured);
+            add_relabels(cs, relabelled);
+            const ChangeSetDev dcs = upload_change_set(h, cs);
+            zero_scalar(h, S_NSEL);
+            if (kind == ListKind::kHash)
+                launch_rebalance_changes_ranked(h->L(), keys, lists, R, d_idx, s->n, h->tabs.tab, dcs, counters, sel, d_nsel, d_moved, d_changed);
+            else if (kind == ListKind::kSpread)
+                launch_rebalance_changes_spread(h->L(), keys, lists, R, d_idx, s->n, h->tabs.tab, dcs, h->spread_tab, counters, sel, d_nsel, d_moved, d_changed);
+            else
+                launch_rebalance_changes_affinity(h->L(), s->feats.as<float>(), s->aff_K, lists, R, d_idx, s->n, h->d_fnode.as<float>(), n_total, dcs,
+                                                  spread ? h->aff_dom.as<uint32_t>() : nullptr, counters, sel, d_nsel, d_moved, d_changed);
+            const uint64_t n_sel = read_scalar(h, S_NSEL);
+            if (n_sel) {   // S1: the selected objects' lists computed afresh, scattered back
+                // the hash kinds on the flat kernels (the solver is HRW here), the affinity kinds on the recorded path
+                h->s_idx.ensure(n_sel * R * 4, h->stream);
+                const void *in;
+                if (affinity) {
+                    h->s_feats.ensure(n_sel * s->aff_K * 4, h->stream);
+                    launch_gather_rows(h->L(), s->feats.as<float>(), s->aff_K, sel, n_sel, h->s_feats.as<float>());
+                    in = h->s_feats.p;
+                } else {
+                    h->s_keys2.ensure(n_sel * 8, h->stream);
+                    launch_gather_keys(h->L(), keys, sel, n_sel, h->s_keys2.as<uint64_t>(), nullptr, nullptr);
+                    in = h->s_keys2.p;
+                }
+                run_lists(h, kind, in, n_sel, R, h->s_idx.as<uint32_t>(), affinity_path(h, s->aff_tensor));
+                launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), sel, n_sel, R, lists, d_idx, counters, n_total, d_moved, d_changed);
+            }
         }
         moved = read_scalar(h, S_MOVED);
         changed = read_scalar(h, S_CHANGED);
     }
-    snapshot_feats(s);
+    if (affinity) snapshot_feats(s);
     if (spread) snapshot_labels(s);
 }
 
@@ -2391,22 +2356,22 @@ void rebalance_affinity_lists(rio_objset *s, const uint32_t *idx, const uint32_t
 
 rio_status rio_cuda_set_assign_ranked(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
-    return guarded(s->h, [&] { set_assign_lists(s, ranks, false); });
+    return guarded(s->h, [&] { set_assign_lists(s, ListKind::kHash, ranks); });
 }
 
 rio_status rio_cuda_set_assign_ranked_spread(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
-    return guarded(s->h, [&] { set_assign_lists(s, ranks, true); });
+    return guarded(s->h, [&] { set_assign_lists(s, ListKind::kSpread, ranks); });
 }
 
 rio_status rio_cuda_set_assign_ranked_affinity(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
-    return guarded(s->h, [&] { set_assign_affinity_lists(s, ranks, false); });
+    return guarded(s->h, [&] { set_assign_lists(s, ListKind::kAffinity, ranks); });
 }
 
 rio_status rio_cuda_set_assign_ranked_affinity_spread(rio_objset *s, uint32_t ranks) {
     if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
-    return guarded(s->h, [&] { set_assign_affinity_lists(s, ranks, true); });
+    return guarded(s->h, [&] { set_assign_lists(s, ListKind::kAffinitySpread, ranks); });
 }
 
 rio_status rio_cuda_set_read_ranked(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out) {
@@ -2427,66 +2392,14 @@ rio_status rio_cuda_set_rebalance_changes_ranked(rio_objset *s, const uint32_t *
     rio_placement *h = s->h;
     return guarded(h, [&] {
         check_change_set(h, idx, prev_weight, k);
-        const bool spread = s->spread;   // the kind of lists the set holds (false when it holds none)
-        if (s->affinity) require_affinity_set_kernels(spread);
-        else if (spread) require_spread_set_kernels(h->solver);
-        else require_ranked_set_kernels(h->solver);
+        require_set_kernels(s->kind, h->solver);   // the hash kind's when the set holds no lists
         REQUIRE(s->ranks, "set holds no ranked lists");
-        if (s->affinity) {   // affinity lists (DESIGN.md 3.15): the solver and trie_bits play no part
+        if (is_affinity(s->kind))   // affinity lists (DESIGN.md 3.15): the solver and trie_bits play no part
             REQUIRE(h->K == s->aff_K, "the set's affinity lists were computed under another node feature K: assign the lists again");
-            uint64_t moved = 0, changed = 0;
-            rebalance_affinity_lists(s, idx, prev_weight, k, moved, changed);
-            if (out_moved) *out_moved = moved;
-            if (out_changed) *out_changed = changed;
-            return;
-        }
-        REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
-        const uint32_t R = s->ranks;
+        else
+            REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
         uint64_t moved = 0, changed = 0;
-        // spread lists: the relabels since the snapshot belong to the change set (DESIGN.md 3.13)
-        const std::vector<uint32_t> relabelled = spread ? relabelled_live(s) : std::vector<uint32_t>{};
-        if (k || !relabelled.empty()) {
-            ensure_tab(h);
-            if (spread) ensure_spread_tab(h);
-            set_ensure_counters(s);
-            zero_scalar(h, S_MOVED);
-            zero_scalar(h, S_CHANGED);
-            uint32_t *lists = s->lists.as<uint32_t>(), *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>();
-            if (h->solver == RIO_SOLVER_HRW2) {   // one ranked re-walk of every key, only the changed rows written
-                if (spread) {
-                    launch_reassign_trie_spread(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->spread_tab, R, lists, d_idx, counters,
-                                                h->tabs.tab.n_total, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-                } else {
-                    ensure_rank_tab(h);
-                    launch_reassign_trie_ranked(h->L(), s->keys.as<uint64_t>(), s->n, h->tabs.trie, h->rank_tab, R, lists, d_idx, counters, h->tabs.tab.n_total,
-                                                h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-                }
-            } else {
-                ChangeSetHost cs = build_change_set(h, idx, prev_weight, k);
-                add_relabels(cs, relabelled);
-                const ChangeSetDev dcs = upload_change_set(h, cs);
-                zero_scalar(h, S_NSEL);
-                if (spread)
-                    launch_rebalance_changes_spread(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, h->spread_tab, counters,
-                                                    s->sel.as<uint32_t>(), h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-                else
-                    launch_rebalance_changes_ranked(h->L(), s->keys.as<uint64_t>(), lists, R, d_idx, s->n, h->tabs.tab, dcs, counters, s->sel.as<uint32_t>(),
-                                                    h->d_scalars + S_NSEL, h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-                const uint64_t n_sel = read_scalar(h, S_NSEL);
-                if (n_sel) {   // S1: the selected objects' lists computed afresh over the live set, scattered back
-                    h->s_keys2.ensure(n_sel * 8, h->stream);
-                    h->s_idx.ensure(n_sel * R * 4, h->stream);
-                    launch_gather_keys(h->L(), s->keys.as<uint64_t>(), s->sel.as<uint32_t>(), n_sel, h->s_keys2.as<uint64_t>(), nullptr, nullptr);
-                    if (spread) launch_assign_hrw_spread(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, h->spread_tab, R, h->s_idx.as<uint32_t>());
-                    else launch_assign_hrw_ranked(h->L(), h->s_keys2.as<uint64_t>(), n_sel, h->tabs.tab, R, h->s_idx.as<uint32_t>());
-                    launch_scatter_ranked(h->L(), h->s_idx.as<uint32_t>(), s->sel.as<uint32_t>(), n_sel, R, lists, d_idx, counters, h->tabs.tab.n_total,
-                                          h->d_scalars + S_MOVED, h->d_scalars + S_CHANGED);
-                }
-            }
-            moved = read_scalar(h, S_MOVED);
-            changed = read_scalar(h, S_CHANGED);
-        }
-        if (spread) snapshot_labels(s);
+        rebalance_lists(s, idx, prev_weight, k, moved, changed);
         if (out_moved) *out_moved = moved;
         if (out_changed) *out_changed = changed;
     });
