@@ -266,6 +266,21 @@ rio_status  rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total
 rio_status  rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k,
                                                             uint64_t n_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
                                                             uint64_t *out_moved, uint32_t *out_passes);
+/* Object churn in a resident set (DESIGN.md 3.18).  rio_cuda_set_insert appends m objects as rows [n, n+m) (*out_first = n, may
+ * be NULL) and places them as the set's current kind places a fresh object: no node while the set is unassigned; the list the
+ * batch call of the set's list kind returns, column 0 as idx, for a set holding ranked lists; the plain affinity argmin on the
+ * recorded path for a bounded affinity record (a later rio_cuda_set_rebalance_changes_bounded_affinity with k = 0 brings the set
+ * back within capacity); otherwise what rio_cuda_assign_batch returns for it (hash: the handle's current policy; affinity: the
+ * recorded path).  feats (m x the set's K) is required exactly when the set has features.  The counters gain the new rows; no
+ * existing row changes.  rio_cuda_set_erase removes every row whose key is one of keys[0..m) (duplicates allowed, absent keys
+ * ignored; *out_erased, may be NULL, = rows removed): with n' the new size, the surviving rows at or above n' fill the removed rows
+ * below n', both in increasing order, carrying key, idx, feature row and list row; nothing else moves.  The counters lose the
+ * removed rows of an assigned set.  Lists, snapshots and records stay; the directory is not touched.  m == 0 does nothing.
+ * RIO_ERR_UNKNOWN (nothing changed): keys NULL with m > 0, features missing or given to a set without them, n + m > capacity, a
+ * bounded call in flight on the set, hash lists computed under another solver or trie_bits, or an affinity kind or record under
+ * another K; RIO_ERR_UPSTREAM when the library was built without the churn kernels. */
+rio_status  rio_cuda_set_insert(rio_objset *s, const uint64_t *keys, const float *feats, uint64_t m, uint64_t *out_first);
+rio_status  rio_cuda_set_erase(rio_objset *s, const uint64_t *keys, uint64_t m, uint64_t *out_erased);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
 /* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied

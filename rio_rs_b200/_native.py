@@ -86,6 +86,8 @@ SIGNATURES = {
     "rio_cuda_set_assign_bounded_end": (C.c_int32, [H, u32p]),
     "rio_cuda_set_assign_bounded_affinity": (C.c_int32, [H, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p]),
     "rio_cuda_set_rebalance_changes_bounded_affinity": (C.c_int32, [H, vp, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u64p, u32p]),
+    "rio_cuda_set_insert": (C.c_int32, [H, vp, vp, C.c_uint64, u64p]),
+    "rio_cuda_set_erase": (C.c_int32, [H, vp, C.c_uint64, u64p]),
     "rio_cuda_set_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),
     "rio_cuda_set_rebalance_changes": (C.c_int32, [H, vp, vp, sz, u64p]),
     "rio_cuda_set_assign_ranked": (C.c_int32, [H, C.c_uint32]),

@@ -13,6 +13,7 @@
 #include "k_affinity_set.cuh"
 #include "k_affinity_bounded.cuh"
 #include "k_set_bounded_affinity.cuh"
+#include "k_set_churn.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -198,6 +199,7 @@ struct rio_placement {
 
     DevBuf s_keys, s_idx, s_idx2, s_sel, s_slots, s_keys2, s_feats, s_packed, s_offsets, s_cost, s_misc, s_flush, s_gather;
     DevBuf s_rows;                            // the spilled objects' feature rows of a bounded affinity round
+    DevBuf s_churn;                           // set_erase (DESIGN.md 3.18): erase-key hash set, row flags, per-block counts and offsets
     // bounded-load state kept on the device between passes (DESIGN.md 3.5): [ticket | cap | global counters | thr | closed epoch | over] x node
     BoundedState bs;                          // for rio_cuda_assign_bounded_batch (host buffers)
     uint64_t tab_version = 0;
@@ -271,6 +273,10 @@ struct rio_objset {
     // bounded-load affinity record (DESIGN.md 3.17): idx is the result of set_assign_bounded_affinity or of the change-set call that
     // keeps it, on the path of aff_tensor under aff_K, with the node features of feat_snap.  Cleared with the lists and by load_feats.
     bool bounded_aff = false;
+    // the plain kind (DESIGN.md 3.18): how the last call that rewrote idx without lists placed it, for set_insert -- by the hash
+    // policy, or by the affinity argmin on the tensor cores (plain_tensor) or the CUDA cores.  Set by set_assign, the bounded assigns
+    // and the set rebalances; left alone by every other call.
+    bool plain_aff = false, plain_tensor = false;
     void drop_lists() { ranks = 0; kind = ListKind::kHash; bounded_aff = false; }
 };
 
@@ -1186,6 +1192,13 @@ void set_zero_counters(rio_objset *s) {
     CUDA_TRY(cudaMemsetAsync(s->counters.p, 0, (size_t)std::max(s->counters_n, 1u) * 4, h->stream));
 }
 
+// the plain kind after an affinity argmin on `path` (DESIGN.md 3.18); with no live node, the path the handle would take for K == 16,
+// as record_affinity decides it
+void record_plain_affinity(rio_objset *s, AffinityPath path) {
+    s->plain_aff = true;
+    s->plain_tensor = path == AffinityPath::kTensorCores || (path == AffinityPath::kNoLiveNode && affinity_umma_wanted());
+}
+
 }  // namespace
 
 // =====================================================================================================================
@@ -1270,7 +1283,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->d_fnode_cm, &h->d_fnode_gm, &h->d_nidx_map_m, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->rank_dev, &h->spread_dev, &h->aff_dom};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->s_churn, &h->rank_dev, &h->spread_dev, &h->aff_dom};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -2007,9 +2020,12 @@ rio_status rio_cuda_set_assign(rio_objset *s, uint32_t use_affinity) {
         set_zero_counters(s);
         if (use_affinity) {
             REQUIRE(s->K > 0 && s->K == h->K, "set features / node features missing or of different K");
-            run_affinity(h, s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), nullptr, s->counters.as<uint32_t>(), affinity_path(h));
+            const AffinityPath path = affinity_path(h);
+            run_affinity(h, s->feats.as<float>(), s->n, s->idx.as<uint32_t>(), nullptr, s->counters.as<uint32_t>(), path);
+            record_plain_affinity(s, path);
         } else {
             run_assign(h, h->solver, h->tabs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), nullptr, 0);
+            s->plain_aff = false;
         }
         s->assigned = true;
     });
@@ -2028,6 +2044,7 @@ static void set_bounded_begin(rio_objset *s, uint64_t n_total_objs, uint32_t cap
     bounded_begin(h, s->bs, s->keys.as<uint64_t>(), s->n, s->idx.as<uint32_t>(), s->counters.as<uint32_t>(), s->counters_n, n_total_objs, cap_num, cap_den, max_rounds,
                   false, zeroed, s->counters_alt.as<uint32_t>(), pipelined);
     s->alt_zero = max_rounds > 1;
+    s->plain_aff = false;
 }
 static uint32_t set_bounded_end(rio_objset *s) {
     rio_placement *h = s->h;
@@ -2084,6 +2101,7 @@ rio_status rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total_
         s->assigned = true;
         if (max_rounds == 1) CUDA_TRY(cudaStreamSynchronize(h->stream));   // otherwise the check's report already ordered the pass before this return
         record_affinity(s, path);
+        record_plain_affinity(s, path);
         s->bounded_aff = true;
         if (out_passes) *out_passes = passes;
     });
@@ -2097,6 +2115,7 @@ rio_status rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, u
         REQUIRE(idx < h->nodes.size(), "node index out of range");
         REQUIRE(s->assigned, "set has no assignment yet");
         s->drop_lists();
+        s->plain_aff = false;
         ensure_tab(h);
         set_ensure_counters(s);
         zero_scalar(h, S_MOVED);
@@ -2131,6 +2150,7 @@ rio_status rio_cuda_set_rebalance_changes(rio_objset *s, const uint32_t *idx, co
         check_change_set(h, idx, prev_weight, k);
         REQUIRE(s->assigned, "set has no assignment yet");
         s->drop_lists();
+        s->plain_aff = false;
         uint64_t moved = 0;
         if (k) {
             ensure_tab(h);
@@ -2450,6 +2470,149 @@ rio_status rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const 
         snapshot_feats(s);
         if (out_moved) *out_moved = moved;
         if (out_passes) *out_passes = passes;
+    });
+}
+
+// ---- object churn in resident sets (DESIGN.md 3.18) ---------------------------------------------------------------------------
+namespace {
+
+void require_churn_kernels() {
+    if (!launch_churn_build || !launch_churn_mark || !launch_churn_pairs || !launch_churn_move)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no set churn kernels (k_set_churn.cuh launchers are not linked)"};
+}
+
+// b grows to hold `need` bytes with its first `keep` bytes kept (DevBuf::ensure keeps nothing); at most `limit` bytes unless need is more
+void grow_keeping(rio_placement *h, DevBuf &b, size_t need, size_t keep, size_t limit) {
+    if (need <= b.bytes) return;
+    DevBuf nb;
+    nb.ensure(std::max(need, std::min(limit, b.bytes + b.bytes / 2)), h->stream);
+    if (keep) CUDA_TRY(cudaMemcpyAsync(nb.p, b.p, keep, cudaMemcpyDeviceToDevice, h->stream));
+    b.release(h->stream);
+    b = nb;
+}
+
+// The m new rows' idx (and list rows) as the set's current kind places a fresh object, computed on the staged keys / feature rows into
+// the handle's scratch, never on the set's columns at row n: the HRW2 walk and the K = 16 kernels read their inputs in 16-byte pieces.
+// Returns the m indices on the device; their counters are added.  Lists go straight to rows [n, n + m) of s->lists.
+const uint32_t *place_new_rows(rio_objset *s, const uint64_t *d_keys, const float *d_feats, uint64_t m) {
+    rio_placement *h = s->h;
+    cudaStream_t st = h->stream;
+    uint32_t *counters = s->counters.as<uint32_t>();
+    h->s_idx.ensure(m * std::max(s->ranks, 1u) * 4, st);
+    uint32_t *out = h->s_idx.as<uint32_t>();
+    if (s->ranks) {   // the batch call of the list kind, over the current table; an affinity kind on its recorded path
+        const ListKind kind = s->kind;
+        const uint32_t R = s->ranks;
+        run_lists(h, kind, is_affinity(kind) ? (const void *)d_feats : (const void *)d_keys, m, R, out, affinity_path(h, s->aff_tensor));
+        CUDA_TRY(cudaMemcpyAsync(s->lists.as<uint32_t>() + s->n * R, out, m * R * 4, cudaMemcpyDeviceToDevice, st));
+        h->s_sel.ensure(m * 4, st);
+        launch_ranked_primary(h->L(), out, m, R, h->s_sel.as<uint32_t>());
+        launch_histogram(h->L(), h->s_sel.as<uint32_t>(), m, counters, s->counters_n);
+        return h->s_sel.as<uint32_t>();
+    }
+    if (s->bounded_aff) run_affinity(h, d_feats, m, out, nullptr, counters, affinity_path(h, s->aff_tensor));
+    else if (s->plain_aff) run_affinity(h, d_feats, m, out, nullptr, counters, affinity_path(h, s->plain_tensor));
+    else run_assign(h, h->solver, h->tabs, d_keys, m, out, counters, nullptr, 0);
+    return out;
+}
+
+}  // namespace
+
+rio_status rio_cuda_set_insert(rio_objset *s, const uint64_t *keys, const float *feats, uint64_t m, uint64_t *out_first) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(keys || !m, "null keys");
+        if (out_first) *out_first = s->n;
+        if (!m) return;
+        REQUIRE(s->K ? feats != nullptr : feats == nullptr, s->K ? "the set has features: insert needs the new rows' features"
+                                                                  : "the set has no features: insert takes none");
+        REQUIRE(m <= s->capacity - s->n, "n + m exceeds the set's capacity");
+        REQUIRE(!s->bs.active, "a bounded call is in flight on this set (call _end first)");
+        require_churn_kernels();
+        const bool lists = s->assigned && s->ranks;
+        if (lists && is_affinity(s->kind))
+            REQUIRE(h->K == s->aff_K, "the set's affinity lists were computed under another node feature K: assign the lists again");
+        else if (lists)
+            REQUIRE(s->rank_solver == h->solver && s->rank_bits == h->trie_bits, "the set's ranked lists were computed under another solver or trie_bits");
+        else if (s->assigned && s->bounded_aff)
+            REQUIRE(h->K == s->aff_K, "the set's bounded affinity assignment was computed under another node feature K: assign it again");
+        else if (s->assigned && s->plain_aff)
+            REQUIRE(h->K == s->K, "the set's affinity assignment was computed under another node feature K: assign it again");
+        if (lists && !launch_ranked_primary)
+            throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no ranked-set kernels (k_ranked_changes.cuh launchers are not linked)"};
+        cudaStream_t st = h->stream;
+        const uint64_t n = s->n;
+        const size_t K = s->K;
+        h->s_keys.ensure(m * 8, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, m * 8, cudaMemcpyHostToDevice, st));
+        if (K) {
+            h->s_feats.ensure(m * K * 4, st);
+            CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, feats, m * K * 4, cudaMemcpyHostToDevice, st));
+            grow_keeping(h, s->feats, (n + m) * K * 4, std::min(s->feats.bytes, n * K * 4), s->capacity * K * 4);
+        }
+        if (s->assigned) {
+            ensure_tab(h);
+            set_ensure_counters(s);
+            const uint32_t *d_new = place_new_rows(s, h->s_keys.as<uint64_t>(), h->s_feats.as<float>(), m);
+            CUDA_TRY(cudaMemcpyAsync(s->idx.as<uint32_t>() + n, d_new, m * 4, cudaMemcpyDeviceToDevice, st));
+        } else {
+            CUDA_TRY(cudaMemsetAsync(s->idx.as<uint32_t>() + n, 0xFF, m * 4, st));   // RIO_NONE
+        }
+        CUDA_TRY(cudaMemcpyAsync(s->keys.as<uint64_t>() + n, h->s_keys.p, m * 8, cudaMemcpyDeviceToDevice, st));
+        if (K) CUDA_TRY(cudaMemcpyAsync(s->feats.as<float>() + n * K, h->s_feats.p, m * K * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        s->n = n + m;
+    });
+}
+
+rio_status rio_cuda_set_erase(rio_objset *s, const uint64_t *keys, uint64_t m, uint64_t *out_erased) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(keys || !m, "null keys");
+        if (out_erased) *out_erased = 0;
+        if (!m) return;
+        REQUIRE(!s->bs.active, "a bounded call is in flight on this set (call _end first)");
+        require_churn_kernels();
+        const uint64_t n = s->n;
+        if (!n) return;
+        cudaStream_t st = h->stream;
+        if (s->assigned) set_ensure_counters(s);
+        // one allocation: the hash set (1 << lg slots, at least 2m), its empty-key flag, then per block of kChurnRows rows the flagged
+        // count, the hole offset and the mover offset, then a flag byte per row
+        uint32_t lg = 6;
+        while ((1ull << lg) < 2 * m) lg++;
+        const uint64_t nb = (n + kChurnRows - 1) / kChurnRows;
+        const size_t o_flag = (size_t)8 << lg, o_cnt = o_flag + 16, o_hoff = o_cnt + nb * 4, o_moff = o_hoff + nb * 4, o_row = o_moff + nb * 4,
+                     total = o_row + n;
+        h->s_churn.ensure(total, st);
+        unsigned char *base = h->s_churn.as<unsigned char>();
+        unsigned long long *table = reinterpret_cast<unsigned long long *>(base);
+        uint32_t *has_empty = reinterpret_cast<uint32_t *>(base + o_flag), *cnt = reinterpret_cast<uint32_t *>(base + o_cnt);
+        CUDA_TRY(cudaMemsetAsync(table, 0xFF, o_flag, st));   // kEmptyKey
+        CUDA_TRY(cudaMemsetAsync(has_empty, 0, 4, st));
+        h->s_keys.ensure(m * 8, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, m * 8, cudaMemcpyHostToDevice, st));
+        launch_churn_build(h->L(), h->s_keys.as<uint64_t>(), m, table, lg, has_empty);
+        zero_scalar(h, S_MOVED);
+        launch_churn_mark(h->L(), s->keys.as<uint64_t>(), s->idx.as<uint32_t>(), n, table, lg, has_empty, s->assigned ? s->counters.as<uint32_t>() : nullptr,
+                          s->counters_n, base + o_row, cnt, h->d_scalars + S_MOVED);
+        const uint64_t erased = read_scalar(h, S_MOVED);
+        const uint64_t n_new = n - erased, max_pairs = std::min(erased, n_new);
+        if (max_pairs) {
+            h->s_idx.ensure(max_pairs * 4, st);
+            h->s_idx2.ensure(max_pairs * 4, st);
+            zero_scalar(h, S_NSEL);
+            launch_churn_pairs(h->L(), base + o_row, n, n_new, cnt, reinterpret_cast<uint32_t *>(base + o_hoff), reinterpret_cast<uint32_t *>(base + o_moff),
+                               h->s_idx.as<uint32_t>(), h->s_idx2.as<uint32_t>(), h->d_scalars + S_NSEL);
+            const bool feats = s->K && s->feats.bytes >= n * (size_t)s->K * 4;   // feature rows that cover the set move with it
+            launch_churn_move(h->L(), h->s_idx.as<uint32_t>(), h->s_idx2.as<uint32_t>(), max_pairs, h->d_scalars + S_NSEL, s->keys.as<uint64_t>(),
+                              s->idx.as<uint32_t>(), s->ranks ? s->lists.as<uint32_t>() : nullptr, s->ranks, feats ? s->feats.as<float>() : nullptr, s->K);
+            CUDA_TRY(cudaStreamSynchronize(st));
+        }
+        s->n = n_new;
+        if (out_erased) *out_erased = erased;
     });
 }
 

@@ -1,6 +1,6 @@
 // k_rank_common.cuh -- launch shape, shared-memory staging, the exact HRW2 contest, the compare-mode epilogue, the warp-aggregated
 // list append and the rank dispatch of the ranked walks (k_ranked.cu, k_spread.cu) and the change-set passes (k_directory.cu,
-// k_affinity_set.cu).
+// k_affinity_set.cu, k_set_bounded_affinity.cu, k_set_churn.cu).
 // Included by .cu files only: everything is internal to the including translation unit.
 #pragma once
 #include "kernels.cuh"
@@ -75,6 +75,14 @@ __device__ __forceinline__ unsigned long long warp_reserve(unsigned long long *n
     unsigned long long b = 0;
     if (lane == 0 && total) b = atomicAdd(n, (unsigned long long)total);
     return __shfl_sync(0xFFFFFFFFu, b, 0) + (pre - mine);
+}
+
+// counters[j] += delta for every lane's j (kNone: none), one atomic per distinct node of the warp: a joined node that many objects of a
+// warp prefer, a leaving node they all held, or an erased rack, costs one atomic.  Every lane of the warp calls this.
+__device__ __forceinline__ void warp_count_add(uint32_t *counters, uint32_t j, uint32_t delta) {
+    if (__ballot_sync(0xFFFFFFFFu, j != kNone) == 0) return;
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, j);
+    if (j != kNone && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicAdd(&counters[j], delta * (uint32_t)__popc(peers));
 }
 
 // Compare mode of the HRW2 walks (DESIGN.md 3.11, 3.13): the output holds the stored lists of a resident set.  Each walk is compared

@@ -9,14 +9,6 @@ namespace rio {
 
 namespace {
 
-// counters[j] += delta for every lane's j (kNone: none), one atomic per distinct node of the warp: a joined node that many objects of a
-// warp prefer, or a leaving node they all held, costs one atomic.  Every lane of the warp calls this.
-__device__ __forceinline__ void warp_count_add(uint32_t *counters, uint32_t j, uint32_t delta) {
-    if (__ballot_sync(0xFFFFFFFFu, j != kNone) == 0) return;
-    const unsigned peers = __match_any_sync(0xFFFFFFFFu, j);
-    if (j != kNone && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicAdd(&counters[j], delta * (uint32_t)__popc(peers));
-}
-
 // Pass 0 of 3.17, in place on idx: 4 B read + 4 B of prev written per object and its node's flag byte; with candidates an S2 object also
 // reads its 4K B of features and costs its node and every candidate (one dot product each).  The trip loop is block-uniform, so the
 // counter updates and the S1 append can ballot.

@@ -588,6 +588,24 @@ class ObjectSet:
                                                                         C.byref(m), C.byref(passes)))
         return m.value, passes.value
 
+    def insert(self, keys, feats=None):
+        """Appends the objects as rows [n, n + len(keys)) and places them as the set's current kind places a fresh object (DESIGN.md
+        3.18); feats (len(keys) x K) exactly when the set has features.  No existing row changes.  Returns the first new row."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        if feats is not None:
+            feats = np.ascontiguousarray(feats, dtype=np.float32)
+        first = C.c_uint64(0)
+        self._ck(self.L.rio_cuda_set_insert(self.s, _ptr(keys), _ptr(feats), len(keys), C.byref(first)))
+        return first.value
+
+    def erase(self, keys):
+        """Removes every row whose key is one of `keys` (DESIGN.md 3.18): the surviving rows past the new end fill the holes, in order;
+        no remaining object changes node or list.  Returns the number of rows removed."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        erased = C.c_uint64(0)
+        self._ck(self.L.rio_cuda_set_erase(self.s, _ptr(keys), len(keys), C.byref(erased)))
+        return erased.value
+
     def assign_bounded_begin(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
         self._ck(self.L.rio_cuda_set_assign_bounded_begin(self.s, n_total, cap_num, cap_den, max_rounds))
 

@@ -96,6 +96,8 @@ extern "C" {
     pub fn rio_cuda_set_assign_bounded_end(s: *mut rio_objset, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_assign_bounded_affinity(s: *mut rio_objset, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_rebalance_changes_bounded_affinity(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_moved: *mut u64, out_passes: *mut u32) -> rio_status;
+    pub fn rio_cuda_set_insert(s: *mut rio_objset, keys: *const u64, feats: *const f32, m: u64, out_first: *mut u64) -> rio_status;
+    pub fn rio_cuda_set_erase(s: *mut rio_objset, keys: *const u64, m: u64, out_erased: *mut u64) -> rio_status;
     pub fn rio_cuda_set_rebalance(s: *mut rio_objset, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_rebalance_changes(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_assign_ranked(s: *mut rio_objset, ranks: u32) -> rio_status;
