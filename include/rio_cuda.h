@@ -151,6 +151,13 @@ rio_status  rio_cuda_assign_bounded_batch(rio_placement *h, const uint64_t *keys
 rio_status  rio_cuda_assign_bounded_affinity_batch(rio_placement *h, const uint64_t *keys, const float *obj_feats, size_t n,
                                                    uint64_t n_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
                                                    uint32_t *out_idx, uint32_t *out_passes);
+/* rio_cuda_set_assign_bounded_weighted for host buffers (DESIGN.md 3.19): keys (n) feed the hash policy and the spill hash;
+ * obj_feats (n x K, K of set_nodes) selects the affinity cost, NULL the hash policy; weights (n) are the objects' loads, NULL = all 1.
+ * Returns exactly what the set call returns for the same rows, with the same refusals (this rank's weight sum is that of `weights`);
+ * also RIO_ERR_UNKNOWN for NULL keys or out_idx.  n == 0 returns at once and takes part in no exchange. */
+rio_status  rio_cuda_assign_bounded_weighted_batch(rio_placement *h, const uint64_t *keys, const float *obj_feats, const uint32_t *weights,
+                                                   size_t n, uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                                                   uint32_t *out_idx, uint32_t *out_passes);
 /* Ranked placement (DESIGN.md 3.9): each object's first `ranks` distinct nodes under the handle's solver policy.  rank 1 is
  * exactly what assign_batch returns; rank r is the same policy's placement over the live set minus ranks 1..r-1 -- so rank 2 is
  * where a LEAVE of rank 1 sends the object (its failover target).  Pure function of (keys, live set); hash path only (the affinity cost: rio_cuda_assign_ranked_affinity_batch).
@@ -281,6 +288,33 @@ rio_status  rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const
  * another K; RIO_ERR_UPSTREAM when the library was built without the churn kernels. */
 rio_status  rio_cuda_set_insert(rio_objset *s, const uint64_t *keys, const float *feats, uint64_t m, uint64_t *out_first);
 rio_status  rio_cuda_set_erase(rio_objset *s, const uint64_t *keys, uint64_t m, uint64_t *out_erased);
+/* Weighted objects (DESIGN.md 3.19).  Every set has one uint32 weight per row, 1 unless written: rio_cuda_set_write_weights writes
+ * rows [first, first+n) from w, rio_cuda_set_read_weights reads them into out (the range must lie inside [0, size)).  The column
+ * (capacity x 4 bytes) is allocated by the first write; a set never written allocates nothing.  set_load_keys and set_synth_keys
+ * reset every weight to 1, set_insert gives each new row weight 1 (write the real weights at *out_first), and set_erase moves each
+ * row's weight with its key; no other call reads or changes them.
+ * rio_cuda_set_assign_bounded_weighted is rio_cuda_set_assign_bounded (use_affinity = 0) or rio_cuda_set_assign_bounded_affinity
+ * (use_affinity = 1) with node LOADS in place of object counts: a node's load is the global sum of the weights of its objects, its
+ * capacity ceil(cap_num * L * w / (cap_den * W)) with L = load_total (0 = G, the weight sum of every rank's shard, reduced across ranks
+ * by one exchange; an explicit load_total must be the same on every rank), and a round spills an object
+ * of weight > 0 from a node over capacity iff its spill hash is below floor(2^32 (load - cap) / load).  Objects of weight 0 never
+ * spill.  Pass 0 is rio_cuda_set_assign(s, use_affinity) bit for bit; a spilled object goes where pass 0's method places it over the
+ * live nodes not closed.  With every weight 1 and load_total = n_total the result (idx, counters, passes) equals the count-based call
+ * bit for bit.  Afterwards the counters are the object counts of the result (not loads), the set records a plain assignment (hash,
+ * or affinity on the path taken) and holds no ranked lists or bounded affinity record.  Loads are u32: the global weight total
+ * must stay below 2^32.  RIO_ERR_UNKNOWN (nothing changed): on each rank before any exchange (pass the same arguments on every rank),
+ * cap_den == 0, max_rounds == 0, use_affinity > 1, a bounded call in flight on the set, the feature errors of
+ * rio_cuda_set_assign_bounded_affinity (use_affinity = 1); on every rank together, after the reduction of G, G or load_total above
+ * 2^32-1, or load_total != 0 below G.
+ * rio_cuda_set_loads copies the global (all ranks, collective as rio_cuda_set_counters is) per-node weight sums of the current
+ * assignment into out (cap >= node count), computed on demand; an unassigned set reports zeros; RIO_ERR_UNKNOWN, on every rank
+ * together, for G above 2^32-1.  RIO_ERR_UPSTREAM for the weighted assign, rio_cuda_set_loads, and set_erase on a set with a weight
+ * column, when the library was built without the weighted kernels. */
+rio_status  rio_cuda_set_write_weights(rio_objset *s, uint64_t first, uint64_t n, const uint32_t *w);
+rio_status  rio_cuda_set_read_weights(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out);
+rio_status  rio_cuda_set_assign_bounded_weighted(rio_objset *s, uint32_t use_affinity, uint64_t load_total, uint32_t cap_num,
+                                                 uint32_t cap_den, uint32_t max_rounds, uint32_t *out_passes);
+rio_status  rio_cuda_set_loads(rio_objset *s, uint32_t *out, uint32_t cap);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
 /* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied

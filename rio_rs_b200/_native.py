@@ -63,6 +63,7 @@ SIGNATURES = {
     "rio_cuda_assign_batch": (C.c_int32, [H, vp, vp, sz, vp]),
     "rio_cuda_assign_bounded_batch": (C.c_int32, [H, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p]),
     "rio_cuda_assign_bounded_affinity_batch": (C.c_int32, [H, vp, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p]),
+    "rio_cuda_assign_bounded_weighted_batch": (C.c_int32, [H, vp, vp, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, vp, u32p]),
     "rio_cuda_assign_ranked_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_batch_dev": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
     "rio_cuda_assign_ranked_spread_batch": (C.c_int32, [H, vp, sz, C.c_uint32, vp]),
@@ -88,6 +89,10 @@ SIGNATURES = {
     "rio_cuda_set_rebalance_changes_bounded_affinity": (C.c_int32, [H, vp, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u64p, u32p]),
     "rio_cuda_set_insert": (C.c_int32, [H, vp, vp, C.c_uint64, u64p]),
     "rio_cuda_set_erase": (C.c_int32, [H, vp, C.c_uint64, u64p]),
+    "rio_cuda_set_write_weights": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp]),
+    "rio_cuda_set_read_weights": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp]),
+    "rio_cuda_set_assign_bounded_weighted": (C.c_int32, [H, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p]),
+    "rio_cuda_set_loads": (C.c_int32, [H, vp, C.c_uint32]),
     "rio_cuda_set_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),
     "rio_cuda_set_rebalance_changes": (C.c_int32, [H, vp, vp, sz, u64p]),
     "rio_cuda_set_assign_ranked": (C.c_int32, [H, C.c_uint32]),

@@ -14,6 +14,7 @@
 #include "k_affinity_bounded.cuh"
 #include "k_set_bounded_affinity.cuh"
 #include "k_set_churn.cuh"
+#include "k_bounded_weighted.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -140,7 +141,7 @@ struct TabBufs {
 
 // device scalars (one small allocation): [0]=nsel [1]=moved/removed [2]=new keys (cumulative) [3]=placed ; u32 error at [8]
 enum { S_NSEL = 0, S_MOVED = 1, S_NEWKEYS = 2, S_PLACED = 3, S_FLAGS = 4 /* host-only: {any over, open nodes} written by k_exchange_check */, S_CHANGED = 5,
-       S_COUNT = 8 };
+       S_WSUM = 6 /* weight sum of a weighted bounded call (DESIGN.md 3.19) */, S_COUNT = 8 };
 
 // Device + host state of one bounded-load call in flight (DESIGN.md 3.5): capacities, global counters, thresholds, closed set,
 // the fused tail's ticket, and three words of mapped pinned memory the capacity check reports into.  Every resident set owns
@@ -200,6 +201,7 @@ struct rio_placement {
     DevBuf s_keys, s_idx, s_idx2, s_sel, s_slots, s_keys2, s_feats, s_packed, s_offsets, s_cost, s_misc, s_flush, s_gather;
     DevBuf s_rows;                            // the spilled objects' feature rows of a bounded affinity round
     DevBuf s_churn;                           // set_erase (DESIGN.md 3.18): erase-key hash set, row flags, per-block counts and offsets
+    DevBuf s_weights;                         // the object weights of rio_cuda_assign_bounded_weighted_batch (DESIGN.md 3.19)
     // bounded-load state kept on the device between passes (DESIGN.md 3.5): [ticket | cap | global counters | thr | closed epoch | over] x node
     BoundedState bs;                          // for rio_cuda_assign_bounded_batch (host buffers)
     uint64_t tab_version = 0;
@@ -277,6 +279,11 @@ struct rio_objset {
     // policy, or by the affinity argmin on the tensor cores (plain_tensor) or the CUDA cores.  Set by set_assign, the bounded assigns
     // and the set rebalances; left alone by every other call.
     bool plain_aff = false, plain_tensor = false;
+    // the weight column (DESIGN.md 3.19): one u32 per row, capacity rows, allocated by the first rio_cuda_set_write_weights; while
+    // has_weights is false every weight is 1 (set_load_keys and set_synth_keys clear it).  loads: M u32 of per-node weight sums.
+    DevBuf weights, loads;
+    bool has_weights = false;
+    const uint32_t *weights_or_null() const { return has_weights ? weights.as<uint32_t>() : nullptr; }
     void drop_lists() { ranks = 0; kind = ListKind::kHash; bounded_aff = false; }
 };
 
@@ -1056,11 +1063,11 @@ void bounded_begin(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, u
 }
 
 // Second half: wait for the check (two words in mapped memory), run the spill rounds it asks for.  Returns the passes run.
-// replace(closed, nsel) re-places the nsel objects of d_sel over live minus closed, adding them to d_counters: hash_replace for the
-// hash policy, the affinity launch of the call's path for 3.16.
-template <class Replace>
-uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, uint64_t n, uint32_t *d_idx, uint32_t *d_counters, uint32_t *d_sel,
-                     Replace &&replace) {
+// select(b, round) appends the spilling objects to d_sel (counted at S_NSEL) and takes them off d_counters: launch_select_spill for the
+// object counts of 3.5, the weighted selection of 3.19 for loads.  replace(closed, nsel) re-places the nsel objects of d_sel over live
+// minus closed and adds them back: hash_replace for the hash policy, the affinity launch of the call's path for 3.16.
+template <class Select, class Replace>
+uint32_t bounded_end(rio_placement *h, BoundedState &bs, uint32_t *d_counters, Select &&select, Replace &&replace) {
     REQUIRE(bs.active, "no bounded call in flight on this set");
     bs.active = false;
     cudaStream_t st = h->stream;
@@ -1075,7 +1082,7 @@ uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys,
         // longer describe the same cluster -- and a node that joined since has no counter slot: refuse, the caller runs the call again.
         REQUIRE(live_signature(h) == bs.live_sig, "the live node set changed between the two halves of a bounded call: run it again");
         zero_scalar(h, S_NSEL);
-        launch_select_spill(h->L(), d_keys, d_idx, n, b.thr, b.over, r, d_sel, h->d_scalars + S_NSEL, d_counters);
+        select(b, r);
         std::vector<uint32_t> ce(M, 0);
         CUDA_TRY(cudaMemcpyAsync(ce.data(), b.closed_epoch, (size_t)M * 4, cudaMemcpyDeviceToHost, st));
         const uint64_t nsel = read_scalar(h, S_NSEL);
@@ -1086,6 +1093,15 @@ uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys,
         if (r + 1 < bs.max_rounds) { order_behind_aux_checks(h); launch_check(h, bs, d_counters, b, M, nullptr, st); }
     }
     return passes;
+}
+
+// the rounds over object counts (3.5, 3.16, 3.17)
+template <class Replace>
+uint32_t bounded_end(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, uint64_t n, uint32_t *d_idx, uint32_t *d_counters, uint32_t *d_sel,
+                     Replace &&replace) {
+    return bounded_end(h, bs, d_counters, [&](const BoundedDev &b, uint32_t r) {
+        launch_select_spill(h->L(), d_keys, d_idx, n, b.thr, b.over, r, d_sel, h->d_scalars + S_NSEL, d_counters);
+    }, replace);
 }
 
 // the spill rounds of 3.5: the handle's policy over the masked table
@@ -1140,6 +1156,72 @@ uint32_t bounded_affinity(rio_placement *h, BoundedState &bs, const uint64_t *d_
     return bounded_end(h, bs, d_keys, n, d_idx, d_counters, d_sel, [&](const std::vector<uint8_t> &closed, uint64_t nsel) {
         affinity_replace(h, path, &closed, d_feats, d_sel, nsel, d_idx, d_counters);
     });
+}
+
+// ---- bounded-load rounds over object weights (DESIGN.md 3.19) -------------------------------------------------------------------
+void require_weighted_kernels() {
+    if (!launch_weight_sum || !launch_load_histogram || !launch_select_spill_weighted || !launch_add_loads_sel)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no weighted bounded kernels (k_bounded_weighted.cuh launchers are not linked)"};
+}
+
+constexpr uint64_t kMaxLoad = 0xFFFFFFFFull;   // loads are u32 sums
+
+// the local weight sum of d_w[0..n) (nullptr: n); a device column costs one 8-byte readback
+uint64_t local_weight_sum(rio_placement *h, const uint32_t *d_w, uint64_t n) {
+    if (!d_w || !n) return n;
+    zero_scalar(h, S_WSUM);
+    launch_weight_sum(h->L(), d_w, n, h->d_scalars + S_WSUM);
+    return read_scalar(h, S_WSUM);
+}
+
+// The weight sum of every rank's shard: with world > 1 one exchange of the counter path (collective; every rank calls it in the same
+// order), the u64 sums cut into four 16-bit pieces so that the u32 sum of each piece over any world size up to 2^16 cannot wrap
+uint64_t global_weight_sum(rio_placement *h, uint64_t local) {
+    if (h->world <= 1) return local;
+    uint32_t piece[8] = {};
+    for (int k = 0; k < 4; k++) piece[k] = (uint32_t)(local >> (16 * k)) & 0xFFFFu;
+    h->s_misc.ensure(sizeof piece, h->stream);
+    uint32_t *d = h->s_misc.as<uint32_t>();
+    CUDA_TRY(cudaMemcpyAsync(d, piece, 16, cudaMemcpyHostToDevice, h->stream));
+    exchange_counters(h, d, d + 4, 4);
+    CUDA_TRY(cudaMemcpyAsync(piece + 4, d + 4, 16, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));
+    uint64_t sum = 0;
+    for (int k = 0; k < 4; k++) sum += (uint64_t)piece[4 + k] << (16 * k);
+    return sum;
+}
+
+// The load total L of a weighted call from the global weight sum: load_total, or that sum when it is 0, refused where a u32 load could
+// overflow.  Every rank decides from the same numbers, so a refusal here is collective.
+uint64_t weighted_load_total(uint64_t global, uint64_t load_total) {
+    REQUIRE(global <= kMaxLoad, "the object weights of all ranks sum past 2^32-1 (loads are u32)");
+    REQUIRE(load_total <= kMaxLoad, "load_total past 2^32-1 (loads are u32)");
+    if (!load_total) return global;
+    REQUIRE(load_total >= global, "load_total is below the weight sum of all ranks");
+    return load_total;
+}
+
+// Pass 0 is the plain assignment (run_assign, or run_affinity on `path`) without counters, then the loads of its result; the rounds
+// of 3.5 then run on d_loads: a spill takes its weight off its node, a re-placed object (counters = nullptr) adds it to its new one.
+// d_w == nullptr: every weight is 1.  The set call and the host-buffer call both come here.
+uint32_t bounded_weighted(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, const uint32_t *d_w, uint64_t n, uint32_t *d_idx,
+                          uint32_t *d_loads, uint32_t M, uint32_t *d_sel, uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                          bool affinity, AffinityPath path) {
+    if (affinity) run_affinity(h, d_feats, n, d_idx, nullptr, nullptr, path);
+    else run_assign(h, h->solver, h->tabs, d_keys, n, d_idx, nullptr, nullptr, 0);
+    CUDA_TRY(cudaMemsetAsync(d_loads, 0, (size_t)std::max(M, 1u) * 4, h->stream));
+    launch_load_histogram(h->L(), d_idx, d_w, n, d_loads, M);
+    bounded_begin(h, bs, d_keys, n, d_idx, d_loads, M, load_total, cap_num, cap_den, max_rounds, true, true, nullptr);
+    const auto hash = hash_replace(h, d_keys, n, d_idx, nullptr, d_sel);
+    return bounded_end(h, bs, d_loads,
+                       [&](const BoundedDev &b, uint32_t r) {
+                           launch_select_spill_weighted(h->L(), d_keys, d_idx, d_w, n, b.thr, b.over, r, d_sel, h->d_scalars + S_NSEL, d_loads);
+                       },
+                       [&](const std::vector<uint8_t> &closed, uint64_t nsel) {
+                           if (affinity) affinity_replace(h, path, &closed, d_feats, d_sel, nsel, d_idx, nullptr);
+                           else hash(closed, nsel);
+                           launch_add_loads_sel(h->L(), d_sel, nsel, d_idx, d_w, d_loads, M);
+                       });
 }
 
 template <class F>
@@ -1283,7 +1365,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->d_fnode_cm, &h->d_fnode_gm, &h->d_nidx_map_m, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->s_churn, &h->rank_dev, &h->spread_dev, &h->aff_dom};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->s_churn, &h->s_weights, &h->rank_dev, &h->spread_dev, &h->aff_dom};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -1631,6 +1713,49 @@ rio_status rio_cuda_assign_bounded_affinity_batch(rio_placement *h, const uint64
     });
 }
 
+rio_status rio_cuda_assign_bounded_weighted_batch(rio_placement *h, const uint64_t *keys, const float *obj_feats, const uint32_t *weights, size_t n,
+                                                  uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, uint32_t *out_idx,
+                                                  uint32_t *out_passes) {
+    if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
+    return guarded(h, [&] {
+        if (out_passes) *out_passes = 0;
+        if (!n) return;
+        REQUIRE(keys && out_idx, "null buffer");
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(n < 0xFFFFFFFFull, "batch too large");
+        if (obj_feats) {
+            REQUIRE(h->K > 0, "assign with object features needs node features");
+            require_bounded_affinity_kernels();
+        }
+        require_weighted_kernels();
+        uint64_t local = n;
+        if (weights) { local = 0; for (size_t i = 0; i < n; i++) local += weights[i]; }
+        const uint64_t L = weighted_load_total(global_weight_sum(h, local), load_total);
+        ensure_tab(h);
+        const uint32_t M = h->tabs.tab.n_total, K = h->K;
+        cudaStream_t st = h->stream;
+        h->s_keys.ensure(n * 8, st);
+        h->s_idx.ensure(n * 4, st);
+        h->s_sel.ensure(n * 4, st);
+        h->s_misc.ensure((size_t)std::max(M, 1u) * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, n * 8, cudaMemcpyHostToDevice, st));
+        if (obj_feats) {
+            h->s_feats.ensure(n * (size_t)K * 4, st);
+            CUDA_TRY(cudaMemcpyAsync(h->s_feats.p, obj_feats, n * (size_t)K * 4, cudaMemcpyHostToDevice, st));
+        }
+        if (weights) {
+            h->s_weights.ensure(n * 4, st);
+            CUDA_TRY(cudaMemcpyAsync(h->s_weights.p, weights, n * 4, cudaMemcpyHostToDevice, st));
+        }
+        const uint32_t passes = bounded_weighted(h, h->bs, h->s_keys.as<uint64_t>(), obj_feats ? h->s_feats.as<float>() : nullptr,
+                                                 weights ? h->s_weights.as<uint32_t>() : nullptr, n, h->s_idx.as<uint32_t>(), h->s_misc.as<uint32_t>(), M,
+                                                 h->s_sel.as<uint32_t>(), L, cap_num, cap_den, max_rounds, obj_feats != nullptr, affinity_path(h));
+        CUDA_TRY(cudaMemcpyAsync(out_idx, h->s_idx.p, n * 4, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (out_passes) *out_passes = passes;
+    });
+}
+
 rio_status rio_cuda_assign_batch_dev(rio_placement *h, const uint64_t *d_keys, const float *d_obj_feats, size_t n, uint32_t *d_out_idx) {
     if (!h) { g_last_error = "null handle"; return RIO_ERR_UNKNOWN; }
     return guarded(h, [&] {
@@ -1970,6 +2095,7 @@ void rio_cuda_set_destroy(rio_objset *s) {
         cudaSetDevice(h->device);
         if (h->aux_stream) cudaStreamSynchronize(h->aux_stream);   // a check of this set may still be in flight
         s->keys.release(h->stream); s->idx.release(h->stream); s->feats.release(h->stream); s->counters.release(h->stream); s->counters_alt.release(h->stream); s->sel.release(h->stream); s->bs.release(h->stream); s->lists.release(h->stream);
+        s->weights.release(h->stream); s->loads.release(h->stream);
         cudaStreamSynchronize(h->stream);
     }
     delete s;
@@ -1981,7 +2107,7 @@ rio_status rio_cuda_set_load_keys(rio_objset *s, const uint64_t *keys, uint64_t 
     return guarded(h, [&] {
         REQUIRE(n <= s->capacity && (keys || !n), "too many keys for this set");
         CUDA_TRY(cudaMemcpyAsync(s->keys.p, keys, n * 8, cudaMemcpyHostToDevice, h->stream));
-        s->n = n; s->assigned = false; s->drop_lists();
+        s->n = n; s->assigned = false; s->drop_lists(); s->has_weights = false;
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
@@ -1992,7 +2118,7 @@ rio_status rio_cuda_set_synth_keys(rio_objset *s, uint64_t first, uint64_t n, ui
     return guarded(h, [&] {
         REQUIRE(n <= s->capacity, "too many keys for this set");
         launch_synth_keys(h->L(), s->keys.as<uint64_t>(), first, n, seed);
-        s->n = n; s->assigned = false; s->drop_lists();
+        s->n = n; s->assigned = false; s->drop_lists(); s->has_weights = false;
     });
 }
 
@@ -2104,6 +2230,93 @@ rio_status rio_cuda_set_assign_bounded_affinity(rio_objset *s, uint64_t n_total_
         record_plain_affinity(s, path);
         s->bounded_aff = true;
         if (out_passes) *out_passes = passes;
+    });
+}
+
+// ---- weighted objects (DESIGN.md 3.19) --------------------------------------------------------------------------------------------
+rio_status rio_cuda_set_write_weights(rio_objset *s, uint64_t first, uint64_t n, const uint32_t *w) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(w || !n, "null weights");
+        REQUIRE(first <= s->n && n <= s->n - first, "range outside the set");
+        if (!n) return;
+        if (!s->has_weights) {   // first write: the column, every row 1
+            s->weights.ensure(s->capacity * 4, h->stream);
+            launch_fill_u32(h->L(), s->weights.as<uint32_t>(), s->n, 1u);
+            s->has_weights = true;
+        }
+        CUDA_TRY(cudaMemcpyAsync(s->weights.as<uint32_t>() + first, w, n * 4, cudaMemcpyHostToDevice, h->stream));
+        CUDA_TRY(cudaStreamSynchronize(h->stream));
+    });
+}
+
+rio_status rio_cuda_set_read_weights(rio_objset *s, uint64_t first, uint64_t n, uint32_t *out) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(out || !n, "null buffer");
+        REQUIRE(first <= s->n && n <= s->n - first, "range outside the set");
+        if (!n) return;
+        if (!s->has_weights) { std::fill(out, out + n, 1u); return; }
+        CUDA_TRY(cudaMemcpyAsync(out, s->weights.as<uint32_t>() + first, n * 4, cudaMemcpyDeviceToHost, h->stream));
+        CUDA_TRY(cudaStreamSynchronize(h->stream));
+    });
+}
+
+rio_status rio_cuda_set_assign_bounded_weighted(rio_objset *s, uint32_t use_affinity, uint64_t load_total, uint32_t cap_num, uint32_t cap_den,
+                                                uint32_t max_rounds, uint32_t *out_passes) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(use_affinity <= 1, "use_affinity must be 0 or 1");
+        REQUIRE(!s->bs.active, "a bounded call is already in flight on this set (call _end first)");
+        if (use_affinity) {
+            REQUIRE(h->K > 0, "assign with object features needs node features");
+            REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+            require_bounded_affinity_kernels();
+        }
+        require_weighted_kernels();
+        const uint32_t *d_w = s->weights_or_null();
+        const uint64_t L = weighted_load_total(global_weight_sum(h, local_weight_sum(h, d_w, s->n)), load_total);
+        s->drop_lists();
+        ensure_tab(h);
+        set_ensure_counters(s);
+        const uint32_t M = s->counters_n;
+        s->loads.ensure((size_t)std::max(M, 1u) * 4, h->stream);
+        const AffinityPath path = affinity_path(h);
+        const uint32_t passes = bounded_weighted(h, s->bs, s->keys.as<uint64_t>(), s->feats.as<float>(), d_w, s->n, s->idx.as<uint32_t>(), s->loads.as<uint32_t>(), M,
+                                                 s->sel.as<uint32_t>(), L, cap_num, cap_den, max_rounds, use_affinity != 0, path);
+        // the counters stay object counts, whatever the rounds balanced
+        set_zero_counters(s);
+        launch_histogram(h->L(), s->idx.as<uint32_t>(), s->n, s->counters.as<uint32_t>(), M);
+        if (use_affinity) record_plain_affinity(s, path);
+        else s->plain_aff = false;
+        s->assigned = true;
+        CUDA_TRY(cudaStreamSynchronize(h->stream));
+        if (out_passes) *out_passes = passes;
+    });
+}
+
+rio_status rio_cuda_set_loads(rio_objset *s, uint32_t *out, uint32_t cap) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        require_weighted_kernels();
+        set_ensure_counters(s);
+        const uint32_t M = s->counters_n;
+        REQUIRE(out && cap >= M, "load buffer too small");
+        if (!M) return;
+        const uint32_t *d_w = s->weights_or_null();
+        REQUIRE(global_weight_sum(h, local_weight_sum(h, d_w, s->n)) <= kMaxLoad, "the object weights of all ranks sum past 2^32-1 (loads are u32)");
+        s->loads.ensure((size_t)M * 4, h->stream);
+        CUDA_TRY(cudaMemsetAsync(s->loads.p, 0, (size_t)M * 4, h->stream));
+        if (s->assigned) launch_load_histogram(h->L(), s->idx.as<uint32_t>(), d_w, s->n, s->loads.as<uint32_t>(), M);
+        h->s_misc.ensure((size_t)M * 4, h->stream);
+        exchange_counters(h, s->loads.as<uint32_t>(), h->s_misc.as<uint32_t>(), M);
+        CUDA_TRY(cudaMemcpyAsync(out, h->s_misc.p, (size_t)M * 4, cudaMemcpyDeviceToHost, h->stream));
+        CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
 
@@ -2561,6 +2774,7 @@ rio_status rio_cuda_set_insert(rio_objset *s, const uint64_t *keys, const float 
         }
         CUDA_TRY(cudaMemcpyAsync(s->keys.as<uint64_t>() + n, h->s_keys.p, m * 8, cudaMemcpyDeviceToDevice, st));
         if (K) CUDA_TRY(cudaMemcpyAsync(s->feats.as<float>() + n * K, h->s_feats.p, m * K * 4, cudaMemcpyDeviceToDevice, st));
+        if (s->has_weights) launch_fill_u32(h->L(), s->weights.as<uint32_t>() + n, m, 1u);   // the caller writes the real weights at n
         CUDA_TRY(cudaStreamSynchronize(st));
         s->n = n + m;
     });
@@ -2575,6 +2789,9 @@ rio_status rio_cuda_set_erase(rio_objset *s, const uint64_t *keys, uint64_t m, u
         if (!m) return;
         REQUIRE(!s->bs.active, "a bounded call is in flight on this set (call _end first)");
         require_churn_kernels();
+        if (s->has_weights && !launch_churn_move_weights)   // the weight column must move with its rows: refuse rather than split them
+            throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no weighted bounded kernels (k_bounded_weighted.cuh launchers are not linked): "
+                                             "erase cannot move the set's weight column"};
         const uint64_t n = s->n;
         if (!n) return;
         cudaStream_t st = h->stream;
@@ -2609,6 +2826,8 @@ rio_status rio_cuda_set_erase(rio_objset *s, const uint64_t *keys, uint64_t m, u
             const bool feats = s->K && s->feats.bytes >= n * (size_t)s->K * 4;   // feature rows that cover the set move with it
             launch_churn_move(h->L(), h->s_idx.as<uint32_t>(), h->s_idx2.as<uint32_t>(), max_pairs, h->d_scalars + S_NSEL, s->keys.as<uint64_t>(),
                               s->idx.as<uint32_t>(), s->ranks ? s->lists.as<uint32_t>() : nullptr, s->ranks, feats ? s->feats.as<float>() : nullptr, s->K);
+            if (s->has_weights)
+                launch_churn_move_weights(h->L(), h->s_idx.as<uint32_t>(), h->s_idx2.as<uint32_t>(), max_pairs, h->d_scalars + S_NSEL, s->weights.as<uint32_t>());
             CUDA_TRY(cudaStreamSynchronize(st));
         }
         s->n = n_new;

@@ -85,6 +85,15 @@ __device__ __forceinline__ void warp_count_add(uint32_t *counters, uint32_t j, u
     if (j != kNone && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicAdd(&counters[j], delta * (uint32_t)__popc(peers));
 }
 
+// loads[j] += w for every lane's (j, w) (kNone: none), one atomic per distinct node of the warp carrying the sum of its lanes' weights
+// (DESIGN.md 3.19).  Every lane of the warp calls this.
+__device__ __forceinline__ void warp_load_add(uint32_t *loads, uint32_t j, uint32_t w) {
+    if (__ballot_sync(0xFFFFFFFFu, j != kNone) == 0) return;
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, j);
+    const uint32_t sum = __reduce_add_sync(peers, w);
+    if (j != kNone && sum && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicAdd(&loads[j], sum);
+}
+
 // Compare mode of the HRW2 walks (DESIGN.md 3.11, 3.13): the output holds the stored lists of a resident set.  Each walk is compared
 // with the stored row, only changed rows are written, and the set's primary index and counters follow column 0.
 struct RankedCmp {

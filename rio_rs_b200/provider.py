@@ -347,6 +347,23 @@ class GpuObjectPlacement:
                                                                C.byref(passes)))
         return out, passes.value
 
+    def assign_bounded_weighted_batch(self, keys, weights=None, obj_feats=None, load_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """Bounded-load rounds over object weights (DESIGN.md 3.19) for host buffers: weights (uint32 per key, None = all 1) are the
+        loads the capacities bound; obj_feats selects the affinity cost, None the hash policy.  Returns (indices, passes), what
+        ObjectSet.assign_bounded_weighted gives for the same rows."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        if weights is not None:
+            weights = np.ascontiguousarray(weights, dtype=np.uint32)
+            assert len(weights) == len(keys)
+        if obj_feats is not None:
+            obj_feats = np.ascontiguousarray(obj_feats, dtype=np.float32)
+            assert obj_feats.ndim == 2 and len(obj_feats) == len(keys)
+        out = np.empty(len(keys), dtype=np.uint32)
+        passes = C.c_uint32(0)
+        self._ck(self.L.rio_cuda_assign_bounded_weighted_batch(self.h, _ptr(keys), _ptr(obj_feats), _ptr(weights), len(keys), load_total, cap_num, cap_den,
+                                                               max_rounds, _ptr(out), C.byref(passes)))
+        return out, passes.value
+
     def place_batch(self, keys, policy="hrw", self_address=None):
         keys = np.ascontiguousarray(keys, dtype=np.uint64)
         out = np.empty(len(keys), dtype=np.uint32)
@@ -605,6 +622,34 @@ class ObjectSet:
         erased = C.c_uint64(0)
         self._ck(self.L.rio_cuda_set_erase(self.s, _ptr(keys), len(keys), C.byref(erased)))
         return erased.value
+
+    def write_weights(self, w, first=0):
+        """Writes the weights of rows [first, first + len(w)) (DESIGN.md 3.19); every other row keeps its weight (1 unless written)."""
+        w = np.ascontiguousarray(w, dtype=np.uint32)
+        self._ck(self.L.rio_cuda_set_write_weights(self.s, first, len(w), _ptr(w)))
+
+    def read_weights(self, first=0, n=None):
+        """The weights of rows [first, first + n) -> uint32."""
+        if n is None:
+            n = self.size() - first
+        out = np.empty(max(n, 0), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_set_read_weights(self.s, first, n, _ptr(out)))
+        return out
+
+    def loads(self):
+        """Global per-node sums of the object weights of the current assignment (collective across ranks, as counters())."""
+        total, _ = self.p.node_count()
+        out = np.zeros(max(total, 1), dtype=np.uint32)
+        self._ck(self.L.rio_cuda_set_loads(self.s, _ptr(out), len(out)))
+        return out[:total]
+
+    def assign_bounded_weighted(self, use_affinity=False, load_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """Bounded-load rounds over the set's object weights (DESIGN.md 3.19): the capacities bound each node's load, the sum of its
+        objects' weights, under the hash policy or (use_affinity) the affinity cost of the set's features.  load_total 0 = the weight
+        sum of every rank's shard (reduced across ranks); an explicit load_total must be the same on every rank.  The counters stay object counts; loads() gives the loads.  Returns the passes run."""
+        passes = C.c_uint32(0)
+        self._ck(self.L.rio_cuda_set_assign_bounded_weighted(self.s, int(use_affinity), load_total, cap_num, cap_den, max_rounds, C.byref(passes)))
+        return passes.value
 
     def assign_bounded_begin(self, n_total=0, cap_num=5, cap_den=4, max_rounds=4):
         self._ck(self.L.rio_cuda_set_assign_bounded_begin(self.s, n_total, cap_num, cap_den, max_rounds))

@@ -62,6 +62,7 @@ extern "C" {
     pub fn rio_cuda_node_count(h: *mut rio_placement, out_total: *mut u32, out_live: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_bounded_batch(h: *mut rio_placement, keys: *const u64, n: usize, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_assign_bounded_affinity_batch(h: *mut rio_placement, keys: *const u64, obj_feats: *const f32, n: usize, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
+    pub fn rio_cuda_assign_bounded_weighted_batch(h: *mut rio_placement, keys: *const u64, obj_feats: *const f32, weights: *const u32, n: usize, load_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_idx: *mut u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_check_address_batch(h: *mut rio_placement, addr_idx: *const u32, n: usize, self_idx: u32, out_verdict: *mut u8, out_cleaned: *mut u64) -> rio_status;
     pub fn rio_cuda_node_state(h: *mut rio_placement, idx: u32, active: *mut i32, weight: *mut u32, malformed: *mut i32) -> rio_status;
     pub fn rio_cuda_node_set_domains(h: *mut rio_placement, idx: *const u32, domain: *const u32, k: size_t) -> rio_status;
@@ -98,6 +99,10 @@ extern "C" {
     pub fn rio_cuda_set_rebalance_changes_bounded_affinity(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, n_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_moved: *mut u64, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_insert(s: *mut rio_objset, keys: *const u64, feats: *const f32, m: u64, out_first: *mut u64) -> rio_status;
     pub fn rio_cuda_set_erase(s: *mut rio_objset, keys: *const u64, m: u64, out_erased: *mut u64) -> rio_status;
+    pub fn rio_cuda_set_write_weights(s: *mut rio_objset, first: u64, n: u64, w: *const u32) -> rio_status;
+    pub fn rio_cuda_set_read_weights(s: *mut rio_objset, first: u64, n: u64, out: *mut u32) -> rio_status;
+    pub fn rio_cuda_set_assign_bounded_weighted(s: *mut rio_objset, use_affinity: u32, load_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_passes: *mut u32) -> rio_status;
+    pub fn rio_cuda_set_loads(s: *mut rio_objset, out: *mut u32, cap: u32) -> rio_status;
     pub fn rio_cuda_set_rebalance(s: *mut rio_objset, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_rebalance_changes(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_assign_ranked(s: *mut rio_objset, ranks: u32) -> rio_status;
