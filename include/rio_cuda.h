@@ -377,6 +377,17 @@ rio_status  rio_cuda_set_read(rio_objset *s, uint64_t first, uint64_t n, uint64_
 rio_status  rio_cuda_set_size(rio_objset *s, uint64_t *out_n);
 /* Write the set's assignment through to the directory (update for every object). */
 rio_status  rio_cuda_set_commit(rio_objset *s);
+/* Delta commit (DESIGN.md 3.20): row i < n is selected iff idx[i] differs from what the directory answers for keys[i] at the start of
+ * the call (RIO_NONE for an absent or removed key, the key normalised as the directory does).  The manifest is the selected rows in
+ * increasing row order, entry j = {out_rows[j] = i, out_keys[j] = keys[i] as stored, out_from[j] = the directory's answer,
+ * out_to[j] = idx[i]}; *out_n = its size.  Each out array may be NULL.  dry_run == 0 upserts the selected rows in row order
+ * (to == RIO_NONE removes the key) and changes nothing else; dry_run == 1 leaves the directory as it was.  For distinct keys the
+ * directory afterwards equals the one rio_cuda_set_commit leaves; with a key in several rows every row is compared with the directory
+ * at the start and the last selected row wins.  Only idx is committed, and the set is not touched.  RIO_ERR_UNKNOWN (directory and
+ * out arrays untouched): a null set, a set with no assignment, a bounded call in flight on the set, or *out_n > cap with any out
+ * array non-NULL (*out_n is written then); RIO_ERR_UPSTREAM when the library was built without the set commit kernels. */
+rio_status  rio_cuda_set_commit_changes(rio_objset *s, uint32_t dry_run, uint64_t cap, uint64_t *out_rows, uint64_t *out_keys, uint32_t *out_from,
+                                        uint32_t *out_to, uint64_t *out_n);
 
 /* ---- multi-GPU: one process per GPU; the only collective is the per-node load-counter all-gather -------- */
 #define RIO_COMM_ID_BYTES 128

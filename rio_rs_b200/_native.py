@@ -105,6 +105,7 @@ SIGNATURES = {
     "rio_cuda_set_read": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp, vp]),
     "rio_cuda_set_size": (C.c_int32, [H, u64p]),
     "rio_cuda_set_commit": (C.c_int32, [H]),
+    "rio_cuda_set_commit_changes": (C.c_int32, [H, C.c_uint32, C.c_uint64, vp, vp, vp, vp, u64p]),
     "rio_cuda_comm_unique_id": (C.c_int32, [vp]),
     "rio_cuda_comm_init": (C.c_int32, [H, C.c_int32, C.c_int32, vp]),
     "rio_cuda_comm_ipc_export": (C.c_int32, [H, C.c_int32, C.c_uint32, vp]),

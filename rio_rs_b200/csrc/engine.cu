@@ -14,6 +14,7 @@
 #include "k_affinity_bounded.cuh"
 #include "k_set_bounded_affinity.cuh"
 #include "k_set_churn.cuh"
+#include "k_set_commit.cuh"
 #include "k_bounded_weighted.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
@@ -201,6 +202,7 @@ struct rio_placement {
     DevBuf s_keys, s_idx, s_idx2, s_sel, s_slots, s_keys2, s_feats, s_packed, s_offsets, s_cost, s_misc, s_flush, s_gather;
     DevBuf s_rows;                            // the spilled objects' feature rows of a bounded affinity round
     DevBuf s_churn;                           // set_erase (DESIGN.md 3.18): erase-key hash set, row flags, per-block counts and offsets
+    DevBuf s_commit, s_manifest;              // set_commit_changes (DESIGN.md 3.20): per-block counts and offsets, from, row flags; the manifest
     DevBuf s_weights;                         // the object weights of rio_cuda_assign_bounded_weighted_batch (DESIGN.md 3.19)
     // bounded-load state kept on the device between passes (DESIGN.md 3.5): [ticket | cap | global counters | thr | closed epoch | over] x node
     BoundedState bs;                          // for rio_cuda_assign_bounded_batch (host buffers)
@@ -1365,7 +1367,7 @@ void rio_cuda_destroy(rio_placement *h) {
     }
     for (TabBufs *tb : {&h->tabs, &h->tabs_masked}) if (tb->stage) cudaFreeHost(tb->stage);
     DevBuf *bufs[] = {&h->tabs.dev, &h->tabs_masked.dev, &h->d_fnode, &h->d_fnode_c, &h->d_fnode_g, &h->d_nidx_map, &h->d_fnode_cm, &h->d_fnode_gm, &h->d_nidx_map_m, &h->s_keys, &h->s_idx, &h->s_idx2, &h->s_sel, &h->s_slots, &h->s_keys2, &h->s_feats,
-                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->s_churn, &h->s_weights, &h->rank_dev, &h->spread_dev, &h->aff_dom};
+                      &h->s_packed, &h->s_offsets, &h->s_cost, &h->s_misc, &h->s_flush, &h->s_gather, &h->s_rows, &h->s_churn, &h->s_commit, &h->s_manifest, &h->s_weights, &h->rank_dev, &h->spread_dev, &h->aff_dom};
     h->bs.release(h->stream);
     for (DevBuf *b : bufs) b->release(h->stream);
     if (h->dir.slots) cudaFreeAsync(h->dir.slots, h->stream);
@@ -2876,6 +2878,54 @@ rio_status rio_cuda_set_commit(rio_objset *s) {
         dir_upsert_dev(h, s->keys.as<uint64_t>(), s->idx.as<uint32_t>(), 0, s->n);
         reconcile_dir_keys(h);
         check_device_error(h);
+    });
+}
+
+rio_status rio_cuda_set_commit_changes(rio_objset *s, uint32_t dry_run, uint64_t cap, uint64_t *out_rows, uint64_t *out_keys, uint32_t *out_from,
+                                       uint32_t *out_to, uint64_t *out_n) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE(s->assigned, "set has no assignment yet");
+        REQUIRE(!s->bs.active, "a bounded call is in flight on this set (call _end first)");
+        if (!launch_commit_diff || !launch_commit_list)
+            throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no set commit kernels (k_set_commit.cuh launchers are not linked)"};
+        const uint64_t n = s->n;
+        const bool want = out_rows || out_keys || out_from || out_to;
+        if (!n) { if (out_n) *out_n = 0; return; }
+        cudaStream_t st = h->stream;
+        // one allocation: per block of kCommitRows rows the selected count and its offset, then per row the directory's answer (written
+        // for selected rows only) and a flag byte
+        const uint64_t nb = (n + kCommitRows - 1) / kCommitRows;
+        const size_t o_off = nb * 4, o_from = (o_off + nb * 4 + 15) & ~(size_t)15, o_flag = o_from + n * 4, total = o_flag + n;
+        h->s_commit.ensure(total, st);
+        unsigned char *base = h->s_commit.as<unsigned char>();
+        uint32_t *cnt = reinterpret_cast<uint32_t *>(base), *off = reinterpret_cast<uint32_t *>(base + o_off), *from = reinterpret_cast<uint32_t *>(base + o_from);
+        uint8_t *flag = base + o_flag;
+        launch_commit_diff(h->L(), h->dir, s->keys.as<uint64_t>(), s->idx.as<uint32_t>(), n, flag, from, cnt, off, h->d_scalars + S_NSEL);
+        const uint64_t m = read_scalar(h, S_NSEL);   // the call's one synchronisation before the write
+        if (out_n) *out_n = m;
+        REQUIRE(!want || m <= cap, "the manifest has more entries than cap (*out_n holds its size)");
+        if (!m || (dry_run && !want)) return;
+        // the manifest: rows (u64), keys (u64), from (u32), to (u32), m entries each
+        h->s_manifest.ensure(m * 24, st);
+        uint64_t *d_rows = h->s_manifest.as<uint64_t>(), *d_keys = d_rows + m;
+        uint32_t *d_from = reinterpret_cast<uint32_t *>(d_keys + m), *d_to = d_from + m;
+        launch_commit_list(h->L(), s->keys.as<uint64_t>(), s->idx.as<uint32_t>(), n, flag, from, cnt, off, d_rows, d_keys, d_from, d_to);
+        if (!dry_run) {   // row order: among selected rows of one key the last wins, as in every upsert batch
+            dir_reserve(h, m);
+            dir_upsert_dev(h, d_keys, d_to, 0, m);
+        }
+        if (out_rows) CUDA_TRY(cudaMemcpyAsync(out_rows, d_rows, m * 8, cudaMemcpyDeviceToHost, st));
+        if (out_keys) CUDA_TRY(cudaMemcpyAsync(out_keys, d_keys, m * 8, cudaMemcpyDeviceToHost, st));
+        if (out_from) CUDA_TRY(cudaMemcpyAsync(out_from, d_from, m * 4, cudaMemcpyDeviceToHost, st));
+        if (out_to) CUDA_TRY(cudaMemcpyAsync(out_to, d_to, m * 4, cudaMemcpyDeviceToHost, st));
+        if (dry_run) {
+            CUDA_TRY(cudaStreamSynchronize(st));
+        } else {
+            reconcile_dir_keys(h);
+            check_device_error(h);
+        }
     });
 }
 

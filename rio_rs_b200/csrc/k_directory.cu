@@ -5,6 +5,7 @@
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread_changes.cuh"
+#include "k_set_commit.cuh"
 #include "k_rank_common.cuh"
 #include "spec.cuh"
 #include "bounded_tail.cuh"
@@ -46,6 +47,20 @@ __global__ void k_dir_init(DirSlot *slots, uint64_t cap) {
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cap; i += (uint64_t)gridDim.x * blockDim.x) p[i] = e;
 }
 
+// The directory's answer for a normalised key whose home slot sl holds x (the first probe, already loaded): the node of its slot,
+// kNone for an absent or removed key.
+__device__ __forceinline__ uint32_t dir_answer(const uint4 *slots, const DirDev &dir, unsigned long long key, uint64_t sl, uint4 x) {
+    uint32_t res = kNone;
+    for (uint64_t probes = 0; probes <= dir.mask; probes++) {
+        const unsigned long long k = ((unsigned long long)x.y << 32) | x.x;
+        if (k == key) { res = x.z; break; }
+        if (k == kEmptyKey) break;
+        sl = (sl + 1) & dir.mask;
+        x = slots[sl];
+    }
+    return res;
+}
+
 // lookup (local.rs:42-49).  Random 16-byte probes are latency bound (ncu: long_scoreboard), so every thread keeps four
 // independent first probes in flight; the rare longer probe sequences are finished one by one afterwards.
 constexpr int kLookupIlp = 4;
@@ -69,18 +84,124 @@ k_dir_lookup(DirDev dir, const uint64_t *__restrict__ keys, uint64_t n, uint32_t
         for (int q = 0; q < kLookupIlp; q++) {
             const uint64_t i = i0 + q * stride;
             if (i >= n) continue;
-            uint32_t res = kNone;
-            uint4 x = v[q];
-            uint64_t sl = s[q];
-            for (uint64_t probes = 0; probes <= dir.mask; probes++) {
-                const unsigned long long k = ((unsigned long long)x.y << 32) | x.x;
-                if (k == key[q]) { res = x.z; break; }
-                if (k == kEmptyKey) break;
-                sl = (sl + 1) & dir.mask;
-                x = slots[sl];
-            }
-            out[i] = res;
+            out[i] = dir_answer(slots, dir, key[q], s[q], v[q]);
         }
+    }
+}
+
+// ---- delta commit of a resident set (DESIGN.md 3.20) ----
+// The diff pass: one block per kCommitRows rows, row lo + q * 256 + t in thread t's q-th probe, so each warp reads 32 consecutive keys
+// and idx per probe round.  As in k_dir_lookup every thread keeps kLookupIlp first probes in flight.  Per row: 8 B of key, 4 B of idx,
+// one probe (a 32-byte sector), one flag byte written; 4 B of `from` for a selected row only, so an unchanged set writes no more.
+static_assert(kCommitRows == 256 * kLookupIlp, "a block of the diff pass is 256 threads x kLookupIlp rows");
+__global__ void __launch_bounds__(256)
+k_commit_diff(DirDev dir, const uint64_t *__restrict__ keys, const uint32_t *__restrict__ idx, uint64_t n, uint8_t *__restrict__ flag,
+              uint32_t *__restrict__ from, uint32_t *__restrict__ block_cnt) {
+    const uint4 *slots = reinterpret_cast<const uint4 *>(dir.slots);
+    const uint64_t i0 = (uint64_t)blockIdx.x * kCommitRows + threadIdx.x;
+    unsigned long long key[kLookupIlp];
+    uint64_t s[kLookupIlp];
+    uint32_t to[kLookupIlp];
+    uint4 v[kLookupIlp];
+#pragma unroll
+    for (int q = 0; q < kLookupIlp; q++) {
+        const uint64_t i = i0 + q * 256;
+        key[q] = norm_key(i < n ? __ldg(keys + i) : 0);
+        to[q] = i < n ? __ldg(idx + i) : kNone;
+        s[q] = home_slot(key[q], dir);
+    }
+#pragma unroll
+    for (int q = 0; q < kLookupIlp; q++) v[q] = slots[s[q]];
+    uint32_t cnt = 0;
+#pragma unroll
+    for (int q = 0; q < kLookupIlp; q++) {
+        const uint64_t i = i0 + q * 256;
+        bool sel = false;
+        if (i < n) {
+            const uint32_t res = dir_answer(slots, dir, key[q], s[q], v[q]);
+            sel = res != to[q];
+            flag[i] = sel ? 1 : 0;
+            if (sel) from[i] = res;
+        }
+        cnt += (uint32_t)__syncthreads_count(sel);
+    }
+    if (threadIdx.x == 0) block_cnt[blockIdx.x] = cnt;
+}
+
+// One block: the exclusive offsets of the blocks' selected counts and their total.  Thread t sums a contiguous run of blocks, so the
+// counts are read twice (8 B per kCommitRows rows).
+__global__ void __launch_bounds__(1024)
+k_commit_scan(const uint32_t *__restrict__ block_cnt, uint64_t nb, uint32_t *__restrict__ block_off, unsigned long long *__restrict__ total) {
+    __shared__ uint32_t ws[32];
+    const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const uint64_t per = (nb + 1023) / 1024, b0 = threadIdx.x * per, b1 = b0 + per < nb ? b0 + per : nb;
+    uint32_t mine = 0;
+    for (uint64_t b = b0; b < b1; b++) mine += __ldg(block_cnt + b);
+    uint32_t x = mine;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, x, o);
+        if (lane >= (unsigned)o) x += t;
+    }
+    if (lane == 31) ws[w] = x;
+    __syncthreads();
+    if (w == 0) {
+        uint32_t y = ws[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, y, o);
+            if (lane >= (unsigned)o) y += t;
+        }
+        ws[lane] = y;
+    }
+    __syncthreads();
+    uint32_t off = x - mine + (w ? ws[w - 1] : 0u);
+    for (uint64_t b = b0; b < b1; b++) {
+        block_off[b] = off;
+        off += __ldg(block_cnt + b);
+    }
+    if (threadIdx.x == 0) *total = ws[31];
+}
+
+// The manifest: one block per kCommitRows rows, with the diff pass's row layout.  Positions come from the block's offset, the selected
+// rows of the earlier probe rounds and warps of the block (ballots), and the thread's rank in its warp, so the manifest is in row order
+// with no atomics.  A block with nothing selected reads only its count.
+__global__ void __launch_bounds__(256)
+k_commit_list(const uint64_t *__restrict__ keys, const uint32_t *__restrict__ idx, uint64_t n, const uint8_t *__restrict__ flag,
+              const uint32_t *__restrict__ from, const uint32_t *__restrict__ block_cnt, const uint32_t *__restrict__ block_off,
+              uint64_t *__restrict__ out_rows, uint64_t *__restrict__ out_keys, uint32_t *__restrict__ out_from, uint32_t *__restrict__ out_to) {
+    __shared__ uint32_t wc[kLookupIlp][8];
+    if (__ldg(block_cnt + blockIdx.x) == 0) return;
+    const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5, below = (1u << lane) - 1u;
+    const uint64_t i0 = (uint64_t)blockIdx.x * kCommitRows + threadIdx.x;
+    bool sel[kLookupIlp];
+    unsigned bal[kLookupIlp];
+#pragma unroll
+    for (int q = 0; q < kLookupIlp; q++) {
+        const uint64_t i = i0 + q * 256;
+        sel[q] = i < n && flag[i] != 0;
+        bal[q] = __ballot_sync(0xFFFFFFFFu, sel[q]);
+        if (lane == 0) wc[q][w] = __popc(bal[q]);
+    }
+    __syncthreads();
+    uint32_t base = __ldg(block_off + blockIdx.x);
+#pragma unroll
+    for (int q = 0; q < kLookupIlp; q++) {
+        uint32_t before = 0, all = 0;
+        for (unsigned u = 0; u < 8; u++) {
+            const uint32_t c = wc[q][u];
+            before += u < w ? c : 0u;
+            all += c;
+        }
+        if (sel[q]) {
+            const uint64_t i = i0 + q * 256;
+            const uint32_t p = base + before + __popc(bal[q] & below);
+            out_rows[p] = i;
+            out_keys[p] = __ldg(keys + i);
+            out_from[p] = __ldg(from + i);
+            out_to[p] = __ldg(idx + i);
+        }
+        base += all;
     }
 }
 
@@ -863,6 +984,22 @@ void launch_dir_init(const Launch &L, DirSlot *slots, uint64_t cap) {
 void launch_dir_lookup(const Launch &L, const DirDev &dir, const uint64_t *d_keys, uint64_t n, uint32_t *d_out) {
     if (!n) return;
     k_dir_lookup<<<grid_for((n + kLookupIlp - 1) / kLookupIlp, 256, L.sm_count, 8), 256, 0, L.stream>>>(dir, d_keys, n, d_out);
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_commit_diff(const Launch &L, const DirDev &dir, const uint64_t *d_keys, const uint32_t *d_idx, uint64_t n, uint8_t *d_flag, uint32_t *d_from,
+                        uint32_t *d_block_cnt, uint32_t *d_block_off, unsigned long long *d_total) {
+    if (!n) return;
+    const uint64_t nb = (n + kCommitRows - 1) / kCommitRows;
+    k_commit_diff<<<(unsigned)nb, 256, 0, L.stream>>>(dir, d_keys, d_idx, n, d_flag, d_from, d_block_cnt);
+    RIO_COUNT_LAUNCH(L);
+    k_commit_scan<<<1, 1024, 0, L.stream>>>(d_block_cnt, nb, d_block_off, d_total);
+    RIO_COUNT_LAUNCH(L);
+}
+void launch_commit_list(const Launch &L, const uint64_t *d_keys, const uint32_t *d_idx, uint64_t n, const uint8_t *d_flag, const uint32_t *d_from,
+                        const uint32_t *d_block_cnt, const uint32_t *d_block_off, uint64_t *d_rows, uint64_t *d_mkeys, uint32_t *d_mfrom, uint32_t *d_mto) {
+    if (!n) return;
+    k_commit_list<<<(unsigned)((n + kCommitRows - 1) / kCommitRows), 256, 0, L.stream>>>(d_keys, d_idx, n, d_flag, d_from, d_block_cnt, d_block_off, d_rows,
+                                                                                       d_mkeys, d_mfrom, d_mto);
     RIO_COUNT_LAUNCH(L);
 }
 void launch_dir_upsert(const Launch &L, const DirDev &dir, const uint64_t *d_keys, const uint32_t *d_idx, uint32_t const_idx, uint64_t n, uint32_t seq_base,

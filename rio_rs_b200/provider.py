@@ -733,3 +733,18 @@ class ObjectSet:
 
     def commit(self):
         self._ck(self.L.rio_cuda_set_commit(self.s))
+
+    def commit_changes(self, dry_run=False, cap=None):
+        """Writes into the directory only the rows whose node differs from what the directory answers for their key (DESIGN.md 3.20)
+        and returns those moves as numpy arrays (rows, keys, from_, to), in row order; from_ is the directory's answer before the call
+        (RIO_NONE: absent), to the set's node (RIO_NONE: the key is removed).  dry_run computes the same manifest and leaves the
+        directory as it was.  cap=None asks for the count first, then calls again with buffers of that size."""
+        n = C.c_uint64(0)
+        if cap is None:
+            self._ck(self.L.rio_cuda_set_commit_changes(self.s, 1, 0, None, None, None, None, C.byref(n)))
+            cap = n.value
+        rows, keys = np.empty(cap, np.uint64), np.empty(cap, np.uint64)
+        from_, to = np.empty(cap, np.uint32), np.empty(cap, np.uint32)
+        self._ck(self.L.rio_cuda_set_commit_changes(self.s, int(bool(dry_run)), cap, _ptr(rows), _ptr(keys), _ptr(from_), _ptr(to), C.byref(n)))
+        m = n.value
+        return rows[:m], keys[:m], from_[:m], to[:m]

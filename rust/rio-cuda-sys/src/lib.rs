@@ -116,6 +116,7 @@ extern "C" {
     pub fn rio_cuda_set_read(s: *mut rio_objset, first: u64, n: u64, out_keys: *mut u64, out_idx: *mut u32) -> rio_status;
     pub fn rio_cuda_set_size(s: *mut rio_objset, out_n: *mut u64) -> rio_status;
     pub fn rio_cuda_set_commit(s: *mut rio_objset) -> rio_status;
+    pub fn rio_cuda_set_commit_changes(s: *mut rio_objset, dry_run: u32, cap: u64, out_rows: *mut u64, out_keys: *mut u64, out_from: *mut u32, out_to: *mut u32, out_n: *mut u64) -> rio_status;
 
     pub fn rio_cuda_comm_unique_id(out_id: *mut u8) -> rio_status;
     pub fn rio_cuda_comm_init(h: *mut rio_placement, rank: i32, world: i32, id: *const u8) -> rio_status;
