@@ -315,6 +315,28 @@ rio_status  rio_cuda_set_read_weights(rio_objset *s, uint64_t first, uint64_t n,
 rio_status  rio_cuda_set_assign_bounded_weighted(rio_objset *s, uint32_t use_affinity, uint64_t load_total, uint32_t cap_num,
                                                  uint32_t cap_den, uint32_t max_rounds, uint32_t *out_passes);
 rio_status  rio_cuda_set_loads(rio_objset *s, uint32_t *out, uint32_t cap);
+/* Weighted bounded sets kept within load capacity (DESIGN.md 3.21).
+ * rio_cuda_set_write_weights_by_key gives every row whose key equals keys[j] the weight w[j] (a key listed several times: its last
+ * occurrence; a key in several rows: every one of them; absent keys are ignored) and reports the rows written in *out_written
+ * (nullable).  The first write allocates the column as rio_cuda_set_write_weights does, every other row 1.  m == 0 does nothing.
+ * RIO_ERR_UNKNOWN (nothing changed): keys or w NULL with m > 0, a bounded call in flight on the set.
+ * rio_cuda_set_rebalance_changes_bounded_weighted keeps a set that rio_cuda_set_assign_bounded_weighted (or this call) placed within
+ * its load capacities after a change set (idx, prev_weight, k as in rio_cuda_rebalance_changes) and after weight or churn changes:
+ * pass 0 is the change-set pass of the recorded kind (flat HRW: 3.10; HRW2: an object on a node that left or lost weight takes its
+ * walk over the live set, any other object moves only to a node that joined or gained weight when its walk lands there; affinity:
+ * the pass 0 of rio_cuda_set_rebalance_changes_bounded_affinity), then the weighted rounds of 3.19 from the loads it leaves, with
+ * capacities from load_total as in rio_cuda_set_assign_bounded_weighted.  An object changes node only if pass 0 re-placed it or a
+ * candidate took it, or it spilled from a node over its load capacity.  *out_moved = objects whose node changed, *out_passes = 1 +
+ * the rounds run; the counters are object counts.  The record is kept by set_insert, set_erase, both weight writes and the commits,
+ * and removed by every call that rewrites idx another way, by set_load_keys / set_synth_keys and, for affinity, set_load_feats.
+ * RIO_ERR_UNKNOWN (nothing changed): on each rank before any exchange, no record, a solver or trie_bits (hash) or node feature K
+ * (affinity) other than the recorded one, missing features, the change-set errors of rio_cuda_rebalance_changes, cap_den == 0,
+ * max_rounds == 0, a bounded call in flight; on every rank together, G or load_total above 2^32-1, or load_total != 0 below G.
+ * RIO_ERR_UPSTREAM for both calls when the library was built without their kernels. */
+rio_status  rio_cuda_set_write_weights_by_key(rio_objset *s, const uint64_t *keys, const uint32_t *w, size_t m, uint64_t *out_written);
+rio_status  rio_cuda_set_rebalance_changes_bounded_weighted(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k,
+                                                            uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                                                            uint64_t *out_moved, uint32_t *out_passes);
 /* Incremental rebalance of the set after the node table changed (call AFTER node_upsert / node_set_active). */
 rio_status  rio_cuda_set_rebalance(rio_objset *s, uint32_t event, uint32_t idx, uint64_t *out_moved);
 /* rio_cuda_rebalance_changes for the set, under the plain policy (capacity bounds of an earlier bounded call are not applied

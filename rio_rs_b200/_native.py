@@ -93,6 +93,8 @@ SIGNATURES = {
     "rio_cuda_set_read_weights": (C.c_int32, [H, C.c_uint64, C.c_uint64, vp]),
     "rio_cuda_set_assign_bounded_weighted": (C.c_int32, [H, C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u32p]),
     "rio_cuda_set_loads": (C.c_int32, [H, vp, C.c_uint32]),
+    "rio_cuda_set_write_weights_by_key": (C.c_int32, [H, vp, vp, sz, u64p]),
+    "rio_cuda_set_rebalance_changes_bounded_weighted": (C.c_int32, [H, vp, vp, sz, C.c_uint64, C.c_uint32, C.c_uint32, C.c_uint32, u64p, u32p]),
     "rio_cuda_set_rebalance": (C.c_int32, [H, C.c_uint32, C.c_uint32, u64p]),
     "rio_cuda_set_rebalance_changes": (C.c_int32, [H, vp, vp, sz, u64p]),
     "rio_cuda_set_assign_ranked": (C.c_int32, [H, C.c_uint32]),

@@ -16,6 +16,7 @@
 #include "k_set_churn.cuh"
 #include "k_set_commit.cuh"
 #include "k_bounded_weighted.cuh"
+#include "k_set_weighted_changes.cuh"
 #include "k_changes.cuh"
 #include "k_ranked_changes.cuh"
 #include "k_spread.cuh"
@@ -286,7 +287,12 @@ struct rio_objset {
     DevBuf weights, loads;
     bool has_weights = false;
     const uint32_t *weights_or_null() const { return has_weights ? weights.as<uint32_t>() : nullptr; }
-    void drop_lists() { ranks = 0; kind = ListKind::kHash; bounded_aff = false; }
+    // weighted-bounded record (DESIGN.md 3.21): idx is the result of set_assign_bounded_weighted or of the change-set call that keeps
+    // it, by the plain kind -- the hash policy of (bw_solver, bw_bits), or the affinity argmin (plain_aff) on the path of aff_tensor
+    // under aff_K with the node features of feat_snap.  Cleared with the lists, and for affinity by load_feats.
+    bool bounded_w = false;
+    uint32_t bw_solver = 0, bw_bits = 0;
+    void drop_lists() { ranks = 0; kind = ListKind::kHash; bounded_aff = false; bounded_w = false; }
 };
 
 namespace {
@@ -1203,14 +1209,11 @@ uint64_t weighted_load_total(uint64_t global, uint64_t load_total) {
     return load_total;
 }
 
-// Pass 0 is the plain assignment (run_assign, or run_affinity on `path`) without counters, then the loads of its result; the rounds
-// of 3.5 then run on d_loads: a spill takes its weight off its node, a re-placed object (counters = nullptr) adds it to its new one.
-// d_w == nullptr: every weight is 1.  The set call and the host-buffer call both come here.
-uint32_t bounded_weighted(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, const uint32_t *d_w, uint64_t n, uint32_t *d_idx,
-                          uint32_t *d_loads, uint32_t M, uint32_t *d_sel, uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
-                          bool affinity, AffinityPath path) {
-    if (affinity) run_affinity(h, d_feats, n, d_idx, nullptr, nullptr, path);
-    else run_assign(h, h->solver, h->tabs, d_keys, n, d_idx, nullptr, nullptr, 0);
+// The loads of the assignment in d_idx, then the rounds of 3.5 on d_loads from it: a spill takes its weight off its node, a re-placed
+// object (counters = nullptr) adds it to its new one -- by the hash policy, or by affinity on `path`.  d_w == nullptr: every weight is 1.
+uint32_t weighted_rounds(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, const uint32_t *d_w, uint64_t n, uint32_t *d_idx,
+                         uint32_t *d_loads, uint32_t M, uint32_t *d_sel, uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                         bool affinity, AffinityPath path) {
     CUDA_TRY(cudaMemsetAsync(d_loads, 0, (size_t)std::max(M, 1u) * 4, h->stream));
     launch_load_histogram(h->L(), d_idx, d_w, n, d_loads, M);
     bounded_begin(h, bs, d_keys, n, d_idx, d_loads, M, load_total, cap_num, cap_den, max_rounds, true, true, nullptr);
@@ -1224,6 +1227,16 @@ uint32_t bounded_weighted(rio_placement *h, BoundedState &bs, const uint64_t *d_
                            else hash(closed, nsel);
                            launch_add_loads_sel(h->L(), d_sel, nsel, d_idx, d_w, d_loads, M);
                        });
+}
+
+// Pass 0 is the plain assignment (run_assign, or run_affinity on `path`) without counters, then the weighted rounds from its result.
+// The set call and the host-buffer call both come here.
+uint32_t bounded_weighted(rio_placement *h, BoundedState &bs, const uint64_t *d_keys, const float *d_feats, const uint32_t *d_w, uint64_t n, uint32_t *d_idx,
+                          uint32_t *d_loads, uint32_t M, uint32_t *d_sel, uint64_t load_total, uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds,
+                          bool affinity, AffinityPath path) {
+    if (affinity) run_affinity(h, d_feats, n, d_idx, nullptr, nullptr, path);
+    else run_assign(h, h->solver, h->tabs, d_keys, n, d_idx, nullptr, nullptr, 0);
+    return weighted_rounds(h, bs, d_keys, d_feats, d_w, n, d_idx, d_loads, M, d_sel, load_total, cap_num, cap_den, max_rounds, affinity, path);
 }
 
 template <class F>
@@ -2134,6 +2147,7 @@ rio_status rio_cuda_set_load_feats(rio_objset *s, const float *feats, uint32_t K
         s->K = K;
         if (is_affinity(s->kind)) s->drop_lists();   // affinity lists are lists of the features just replaced; hash lists stay
         s->bounded_aff = false;
+        if (s->plain_aff) s->bounded_w = false;
         CUDA_TRY(cudaStreamSynchronize(h->stream));
     });
 }
@@ -2297,6 +2311,10 @@ rio_status rio_cuda_set_assign_bounded_weighted(rio_objset *s, uint32_t use_affi
         else s->plain_aff = false;
         s->assigned = true;
         CUDA_TRY(cudaStreamSynchronize(h->stream));
+        if (use_affinity) record_affinity(s, path);
+        s->bounded_w = true;
+        s->bw_solver = h->solver;
+        s->bw_bits = h->trie_bits;
         if (out_passes) *out_passes = passes;
     });
 }
@@ -2683,6 +2701,151 @@ rio_status rio_cuda_set_rebalance_changes_bounded_affinity(rio_objset *s, const 
         launch_count_diff(h->L(), d_idx, d_prev, n, h->d_scalars + S_MOVED);
         const uint64_t moved = read_scalar(h, S_MOVED);
         snapshot_feats(s);
+        if (out_moved) *out_moved = moved;
+        if (out_passes) *out_passes = passes;
+    });
+}
+
+// ---- weighted bounded sets kept within load capacity (DESIGN.md 3.21) -----------------------------------------------------------
+namespace {
+
+void require_weight_key_kernels() {
+    if (!launch_weight_keys_build || !launch_weight_keys_apply)
+        throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no weighted change-set kernels (k_set_weighted_changes.cuh launchers are not linked)"};
+}
+
+// The HRW2 change set of 3.21, by weight: REPLACE is every interned node not live now (ChangeSetHost) and every changed live node that
+// lost weight; CANDIDATES every changed live node that joined (prev_weight 0) or gained weight.
+ChangeSetHost build_walk_change_set(const rio_placement *h, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
+    ChangeSetHost cs(h);
+    for (size_t i = 0; i < k; i++) {
+        const NodeInfo &ni = h->nodes[idx[i]];
+        if (!ni.live()) continue;   // REPLACE already
+        if (prev_weight[i] && ni.weight < prev_weight[i]) cs.mark(idx[i], kChgReplace);
+        else if (!prev_weight[i] || ni.weight > prev_weight[i]) cs.mark(idx[i], kChgCandidate);
+    }
+    return cs;
+}
+
+// Pass 0 under the hash policy, on the set's idx (counters not kept: the caller rebuilds them).  Flat HRW: R1 / R2 of 3.10.  HRW2 with
+// candidates: one walk of every key into s_idx2, merged by launch_merge_walk_changes; without: the S1 objects selected and walked.
+void hash_changes_pass0(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k) {
+    rio_placement *h = s->h;
+    const bool trie = h->solver == RIO_SOLVER_HRW2;
+    const ChangeSetHost cs = trie ? build_walk_change_set(h, idx, prev_weight, k) : build_change_set(h, idx, prev_weight, k);
+    const ChangeSetDev dcs = upload_change_set(h, cs);
+    const uint64_t n = s->n;
+    const uint64_t *keys = s->keys.as<uint64_t>();
+    uint32_t *d_idx = s->idx.as<uint32_t>(), *d_sel = s->sel.as<uint32_t>();
+    h->s_idx2.ensure(std::max<uint64_t>(n, 1) * 4, h->stream);   // the walk of every key, or the old node of each selected object
+    if (trie && cs.n_cand) {
+        run_assign(h, RIO_SOLVER_HRW2, h->tabs, keys, n, h->s_idx2.as<uint32_t>(), nullptr, nullptr, 0);
+        launch_merge_walk_changes(h->L(), d_idx, h->s_idx2.as<uint32_t>(), n, dcs.flag, h->tabs.tab.n_total);
+        return;
+    }
+    zero_scalar(h, S_NSEL);
+    launch_rebalance_changes(h->L(), keys, d_idx, n, h->tabs.tab, dcs, nullptr, d_sel, h->s_idx2.as<uint32_t>(), h->d_scalars + S_NSEL, h->d_scalars + S_MOVED);
+    const uint64_t n_sel = read_scalar(h, S_NSEL);
+    if (n_sel) run_assign(h, h->solver, h->tabs, keys, n, d_idx, nullptr, d_sel, n_sel);
+}
+
+}  // namespace
+
+rio_status rio_cuda_set_write_weights_by_key(rio_objset *s, const uint64_t *keys, const uint32_t *w, size_t m, uint64_t *out_written) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        REQUIRE((keys && w) || !m, "null keys or weights");
+        REQUIRE(!s->bs.active, "a bounded call is in flight on this set (call _end first)");
+        if (out_written) *out_written = 0;
+        if (!m) return;
+        require_weight_key_kernels();
+        REQUIRE(m < 0xFFFFFFFFull, "too many keys (positions are u32)");
+        cudaStream_t st = h->stream;
+        // one allocation: the table's keys (1 << lg slots, at least 2m), their positions, then the position of a key equal to ~0
+        uint32_t lg = 6;
+        while ((1ull << lg) < 2 * (uint64_t)m) lg++;
+        const size_t o_pos = (size_t)8 << lg, o_empty = o_pos + ((size_t)4 << lg);
+        h->s_churn.ensure(o_empty + 16, st);
+        unsigned char *base = h->s_churn.as<unsigned char>();
+        CUDA_TRY(cudaMemsetAsync(base, 0xFF, o_pos, st));   // kEmptyKey
+        CUDA_TRY(cudaMemsetAsync(base + o_pos, 0, o_empty + 16 - o_pos, st));
+        h->s_keys.ensure(m * 8, st);
+        h->s_weights.ensure(m * 4, st);
+        CUDA_TRY(cudaMemcpyAsync(h->s_keys.p, keys, m * 8, cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(h->s_weights.p, w, m * 4, cudaMemcpyHostToDevice, st));
+        if (!s->has_weights) {   // first write: the column, every row 1, as set_write_weights allocates it
+            s->weights.ensure(s->capacity * 4, st);
+            launch_fill_u32(h->L(), s->weights.as<uint32_t>(), s->n, 1u);
+            s->has_weights = true;
+        }
+        unsigned long long *table = reinterpret_cast<unsigned long long *>(base);
+        uint32_t *pos = reinterpret_cast<uint32_t *>(base + o_pos), *empty_pos = reinterpret_cast<uint32_t *>(base + o_empty);
+        launch_weight_keys_build(h->L(), h->s_keys.as<uint64_t>(), m, table, pos, lg, empty_pos);
+        zero_scalar(h, S_MOVED);
+        launch_weight_keys_apply(h->L(), s->keys.as<uint64_t>(), s->n, table, pos, lg, empty_pos, h->s_weights.as<uint32_t>(), s->weights.as<uint32_t>(),
+                                 h->d_scalars + S_MOVED);
+        const uint64_t written = read_scalar(h, S_MOVED);
+        if (out_written) *out_written = written;
+    });
+}
+
+rio_status rio_cuda_set_rebalance_changes_bounded_weighted(rio_objset *s, const uint32_t *idx, const uint32_t *prev_weight, size_t k, uint64_t load_total,
+                                                          uint32_t cap_num, uint32_t cap_den, uint32_t max_rounds, uint64_t *out_moved, uint32_t *out_passes) {
+    if (!s) { g_last_error = "null set"; return RIO_ERR_UNKNOWN; }
+    rio_placement *h = s->h;
+    return guarded(h, [&] {
+        // argument errors, decided on each rank before any exchange
+        REQUIRE(s->bounded_w, "set holds no weighted bounded assignment (set_assign_bounded_weighted first)");
+        const bool affinity = s->plain_aff;
+        if (affinity) {
+            REQUIRE(h->K == s->aff_K, "the set's weighted bounded assignment was computed under another node feature K: assign it again");
+            REQUIRE(s->K > 0 && s->K == h->K && s->feats.bytes >= s->n * (size_t)s->K * 4, "set features / node features missing or of different K");
+        } else {
+            REQUIRE(s->bw_solver == h->solver && s->bw_bits == h->trie_bits, "the set's weighted bounded assignment was computed under another solver or trie_bits");
+        }
+        check_change_set(h, idx, prev_weight, k);
+        REQUIRE(cap_den > 0 && max_rounds > 0, "bad capacity factor / rounds");
+        REQUIRE(!s->bs.active, "a bounded call is already in flight on this set (call _end first)");
+        require_weighted_kernels();
+        if (!launch_merge_walk_changes || !launch_rebalance_changes || !launch_count_diff || (affinity && !launch_rebalance_changes_bounded_affinity))
+            throw RioError{RIO_ERR_UPSTREAM, "this build of the engine has no weighted change-set kernels (k_set_weighted_changes.cuh, k_changes.cuh or "
+                                             "k_set_bounded_affinity.cuh launchers are not linked)"};
+        if (affinity) require_bounded_affinity_kernels();
+        // range errors, decided from the global weight sum, so that every rank refuses together
+        const uint32_t *d_w = s->weights_or_null();
+        const uint64_t L = weighted_load_total(global_weight_sum(h, local_weight_sum(h, d_w, s->n)), load_total);
+        ensure_tab(h);
+        set_ensure_counters(s);   // a join may have interned a node
+        const uint64_t n = s->n;
+        const uint32_t M = s->counters_n;
+        s->loads.ensure((size_t)std::max(M, 1u) * 4, h->stream);
+        uint32_t *d_idx = s->idx.as<uint32_t>(), *counters = s->counters.as<uint32_t>(), *d_sel = s->sel.as<uint32_t>();
+        const float *d_feats = s->feats.as<float>();
+        h->s_idx.ensure(std::max<uint64_t>(n, 1) * 4, h->stream);   // each object's node before the call
+        uint32_t *d_prev = h->s_idx.as<uint32_t>();
+        const AffinityPath path = affinity ? affinity_path(h, s->aff_tensor) : affinity_path(h);
+        if (affinity) {   // pass 0 of 3.17: the change set of 3.15 with the refeatured live nodes, S2 in place, S1 over the live set
+            ChangeSetHost cs = build_affinity_change_set(h, idx, prev_weight, k);
+            add_relabels(cs, refeatured_live(s));
+            const ChangeSetDev dcs = upload_change_set(h, cs);
+            zero_scalar(h, S_NSEL);
+            launch_rebalance_changes_bounded_affinity(h->L(), d_feats, s->aff_K, d_idx, d_prev, n, h->d_fnode.as<float>(), h->tabs.tab.n_total, dcs, counters,
+                                                      d_sel, h->d_scalars + S_NSEL);
+            affinity_replace(h, path, nullptr, d_feats, d_sel, read_scalar(h, S_NSEL), d_idx, counters);
+        } else {
+            CUDA_TRY(cudaMemcpyAsync(d_prev, d_idx, n * 4, cudaMemcpyDeviceToDevice, h->stream));
+            if (k) hash_changes_pass0(s, idx, prev_weight, k);
+        }
+        const uint32_t passes = weighted_rounds(h, s->bs, s->keys.as<uint64_t>(), d_feats, d_w, n, d_idx, s->loads.as<uint32_t>(), M, d_sel, L, cap_num, cap_den,
+                                                max_rounds, affinity, path);
+        // the counters stay object counts, whatever the rounds balanced
+        set_zero_counters(s);
+        launch_histogram(h->L(), d_idx, n, counters, M);
+        zero_scalar(h, S_MOVED);
+        launch_count_diff(h->L(), d_idx, d_prev, n, h->d_scalars + S_MOVED);
+        const uint64_t moved = read_scalar(h, S_MOVED);
+        if (affinity) snapshot_feats(s);
         if (out_moved) *out_moved = moved;
         if (out_passes) *out_passes = passes;
     });

@@ -2,6 +2,7 @@
 // hole/mover pairing and the row moves.  In a translation unit of its own, so that no existing kernel's code depends on it.
 #include "kernels.cuh"
 #include "k_set_churn.cuh"
+#include "k_key_probe.cuh"
 #include "k_rank_common.cuh"
 
 namespace rio {
@@ -9,8 +10,6 @@ namespace rio {
 namespace {
 
 constexpr int kScanThreads = 1024;
-
-__device__ __forceinline__ uint64_t churn_slot(unsigned long long key, uint32_t lg) { return (key * kChurnHashMul) >> (64 - lg); }
 
 // one thread per erase key; duplicates find their own key and stop
 __global__ void __launch_bounds__(256)

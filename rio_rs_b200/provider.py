@@ -636,6 +636,26 @@ class ObjectSet:
         self._ck(self.L.rio_cuda_set_read_weights(self.s, first, n, _ptr(out)))
         return out
 
+    def write_weights_by_key(self, keys, w):
+        """Writes weight w[j] into every row whose key is keys[j] (DESIGN.md 3.21): the last occurrence of a repeated key wins, absent
+        keys are ignored.  Returns the rows written."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint64)
+        w = np.ascontiguousarray(w, dtype=np.uint32)
+        assert len(keys) == len(w)
+        out = C.c_uint64(0)
+        self._ck(self.L.rio_cuda_set_write_weights_by_key(self.s, _ptr(keys), _ptr(w), len(keys), C.byref(out)))
+        return out.value
+
+    def rebalance_changes_bounded_weighted(self, idx, prev_weight, load_total=0, cap_num=5, cap_den=4, max_rounds=4):
+        """Keeps the assignment of assign_bounded_weighted within its load capacities after a change set, weight writes or churn
+        (DESIGN.md 3.21): one change-set pass of the recorded kind, then the weighted capacity rounds from the current assignment.
+        Returns (moved, passes): objects whose node changed, and 1 + the rounds run."""
+        idx, prev = _change_set(idx, prev_weight)
+        m, passes = C.c_uint64(0), C.c_uint32(0)
+        self._ck(self.L.rio_cuda_set_rebalance_changes_bounded_weighted(self.s, _ptr(idx), _ptr(prev), len(idx), load_total, cap_num, cap_den, max_rounds,
+                                                                        C.byref(m), C.byref(passes)))
+        return m.value, passes.value
+
     def loads(self):
         """Global per-node sums of the object weights of the current assignment (collective across ranks, as counters())."""
         total, _ = self.p.node_count()

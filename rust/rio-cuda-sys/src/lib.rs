@@ -103,6 +103,8 @@ extern "C" {
     pub fn rio_cuda_set_read_weights(s: *mut rio_objset, first: u64, n: u64, out: *mut u32) -> rio_status;
     pub fn rio_cuda_set_assign_bounded_weighted(s: *mut rio_objset, use_affinity: u32, load_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_loads(s: *mut rio_objset, out: *mut u32, cap: u32) -> rio_status;
+    pub fn rio_cuda_set_write_weights_by_key(s: *mut rio_objset, keys: *const u64, w: *const u32, m: usize, out_written: *mut u64) -> rio_status;
+    pub fn rio_cuda_set_rebalance_changes_bounded_weighted(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: usize, load_total: u64, cap_num: u32, cap_den: u32, max_rounds: u32, out_moved: *mut u64, out_passes: *mut u32) -> rio_status;
     pub fn rio_cuda_set_rebalance(s: *mut rio_objset, event: u32, idx: u32, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_rebalance_changes(s: *mut rio_objset, idx: *const u32, prev_weight: *const u32, k: size_t, out_moved: *mut u64) -> rio_status;
     pub fn rio_cuda_set_assign_ranked(s: *mut rio_objset, ranks: u32) -> rio_status;
